@@ -44,6 +44,8 @@ REASON_HTTP = {
 }
 
 RESP_STREAM, RESP_END_OF_STREAM, RESP_COMPLETED = 1, 2, 4
+RESP_METERED = 8    # a chunk of a metered stream (N5, arks_set_stream_metering); with RESP_STREAM
+FLAG_METERED = 2    # arks_request_result.flags: admitted and metered; the host sets RESP_METERED on its chunks
 # metric row layout (include/arks_gateway.h ARKS_METRIC_*)
 METRIC_COLS, METRIC_HITS, METRIC_USAGE, METRIC_HIST_IN, METRIC_HIST_OUT, METRIC_HIST_BUCKETS, METRIC_MESSAGES = 44, 0, 4, 6, 24, 18, 42
 

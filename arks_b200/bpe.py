@@ -6,7 +6,8 @@
                                  Unicode class table of the Qwen2 split pattern (arks_b200/data/bpe_unicode.bin.z) and
                                  whether the tokenizer normalises to NFC
   content_strings(body)          what is counted: every string that is the value of a key named `content` (the messages of
-                                 a chat request, the message / delta of a completion), JSON escapes decoded
+                                 a chat request, the message / delta of a completion), JSON escapes decoded; with
+                                 keys=METERED_KEYS the wider set metered streams count (N5, arks_set_stream_metering)
   standin_tokenizer(n, seed)     a seeded byte-level BPE trained offline with `tokenizers` on synthetic text, used where
                                  the real Qwen2.5 vocabulary would be (it is not on disk and there is no network): same
                                  pre-tokenizer pattern, same algorithm, ~151 k merges at full scale. TEST / BENCH helper.
@@ -31,6 +32,9 @@ QWEN2_PATTERN = (r"""(?i:'s|'t|'re|'ve|'m|'ll|'d)|[^\r\n\p{L}\p{N}]?\p{L}+|\p{N}
                  r"""|\s+(?!\S)|\s+""")
 BPE_NFC = 1            # arks_bpe_tables.flags
 UNCOUNTED = 0xFFFFFFFF  # ARKS_BPE_UNCOUNTED
+CONTENT_KEYS = ("content",)
+# metered rows (N5): also content parts ({"type":"text","text":..}), reasoning streams and tool-call arguments
+METERED_KEYS = ("content", "text", "reasoning_content", "arguments")
 
 
 def bytes_to_unicode():
@@ -103,13 +107,13 @@ def load_tokenizer(src, merges_txt: str | None = None) -> BpeTables:
     return BpeTables(byte_id, left, right, merged, unicode_classes(), flags)
 
 
-def content_strings(body: bytes) -> list[str]:
-    """every string value of a key named `content`, in document order (duplicated keys included)"""
+def content_strings(body: bytes, keys=CONTENT_KEYS) -> list[str]:
+    """every string value of a key named `content` (or any of `keys`), in document order (duplicated keys included)"""
     out = []
 
     def pairs(ps):
         for k, v in ps:
-            if k == "content" and isinstance(v, str):
+            if k in keys and isinstance(v, str):
                 out.append(v)
         return None
 
@@ -117,13 +121,13 @@ def content_strings(body: bytes) -> list[str]:
     return out
 
 
-def sse_content_strings(chunk: bytes) -> list[str]:
+def sse_content_strings(chunk: bytes, keys=CONTENT_KEYS) -> list[str]:
     """the same over the `data:` lines of an SSE chunk (events that are not JSON carry no text)"""
     out = []
     for line in chunk.replace(b"\r\n", b"\n").split(b"\n"):
         if line.startswith(b"data:"):
             try:
-                out += content_strings(line[5:].strip())
+                out += content_strings(line[5:].strip(), keys)
             except ValueError:
                 pass
     return out

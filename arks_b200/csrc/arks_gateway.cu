@@ -139,6 +139,7 @@ struct ReqDev {  // request batch, device resident
   uint32_t* model_len;  // bit 31: the span contains a backslash
   uint32_t* bpe;        // BPE tokens of the prompt text (0 without a vocabulary)
   int precharge;  // N4: admitted requests charge their BPE count to the token-type rules
+  int meter;      // N5: stream requests without include_usage are decided and metered instead of refused
 };
 
 struct RespDev {
@@ -479,6 +480,9 @@ __device__ __forceinline__ void resolve_request(const DevTables& T, const ReqDev
                                                 uint8_t pstate, uint32_t m_start, uint32_t m_rawlen, uint32_t m_esc) {
   uint8_t reason = ARKS_R_OK, flags = 0, claimer = 0;
   int32_t qos = -1, slot = -1, tok_seen = -1;  // the token is only reported once the decision reached GetQosByToken
+  // N5: a stream without include_usage is metered. The bit is set whatever the decision (the BPE scan counts the wide key
+  // set for it); limit_admit reports it only on admitted rows
+  const uint8_t metered = B.meter && (pstate & (PS_BAD | PS_STREAM | PS_STREAM_OK)) == PS_STREAM ? ARKS_FLAG_METERED : 0;
   do {
     if (pstate & PS_BAD) { reason = ARKS_R_REQUEST_BODY; break; }            // handle_request.go:97-104
     if (m_rawlen == 0) { reason = ARKS_R_NO_MODEL; break; }                  // :106-115
@@ -489,7 +493,7 @@ __device__ __forceinline__ void resolve_request(const DevTables& T, const ReqDev
     if (qos < 0) { reason = ARKS_R_MODEL_NOT_IN_TOKEN; break; }
     if (T.qos_ep[qos] < 0) { reason = ARKS_R_NO_MODEL_BACKENDS; break; }   // handle_request.go:137-154
     const bool stream = pstate & PS_STREAM;
-    if (stream && !(pstate & PS_STREAM_OK)) { reason = ARKS_R_STREAM_OPTIONS; break; }  // :156-171
+    if (stream && !(pstate & PS_STREAM_OK) && !metered) { reason = ARKS_R_STREAM_OPTIONS; break; }  // :156-171
     flags = stream ? 1 : 0;
     // register in the batch-local group table: qos -> dense slot, arrival count, member list
     uint32_t g = ((uint32_t)qos * 2654435761u) & B.gmask;
@@ -512,7 +516,7 @@ __device__ __forceinline__ void resolve_request(const DevTables& T, const ReqDev
     slot = (int32_t)g;
   } while (0);
   B.st_reason[i] = reason;
-  B.st_flags[i] = flags | (claimer << 7);
+  B.st_flags[i] = flags | metered | (claimer << 7);
   B.st_qos[i] = qos;
   B.st_tok[i] = tok_seen;
   B.gslot[i] = slot;
@@ -1271,7 +1275,9 @@ __global__ void __launch_bounds__(128) limit_admit_kernel(DevTables T, ReqDev B)
         else { reason = ARKS_R_QUOTA; detail = (uint8_t)quota_fail; cur_out = q_cur; lim_out = q_lim; }
       }
     }
-    if (admitted && B.precharge) {  // N4 (opt-in): the estimate is charged when the micro-batch commits; nobody reads T.rate here
+    // N4 (opt-in): the estimate is charged when the micro-batch commits; nobody reads T.rate here. Metered rows (N5) are
+    // charged by meter_charge_kernel instead
+    if (admitted && B.precharge && !(B.st_flags[i] & ARKS_FLAG_METERED)) {
       const uint32_t est = B.bpe[i] == kBpeUncounted ? 0u : B.bpe[i];
       if (est && cnt[2]) atomicAdd(reinterpret_cast<unsigned long long*>(T.rate + (size_t)2 * T.n_qos + qos), (unsigned long long)est * (unsigned long long)cnt[2]);
       if (est && cnt[3]) atomicAdd(reinterpret_cast<unsigned long long*>(T.rate + (size_t)3 * T.n_qos + qos), (unsigned long long)est * (unsigned long long)cnt[3]);
@@ -1365,6 +1371,8 @@ __device__ __forceinline__ void account_usage(const DevTables& T, const RespDev&
   if (live && qos < 0) {  // the row's qos entry does not exist in these tables: nothing to bill (ARKS_R_QOS_GONE)
     reason = ARKS_R_QOS_GONE; counted = 0; u0 = u1 = u2 = 0;
   }
+  // N5: a metered stream is billed by meter_charge_kernel; its upstream usage is reported, not billed
+  if (live && (B.flags[i] & (ARKS_RESP_STREAM | ARKS_RESP_METERED)) == (ARKS_RESP_STREAM | ARKS_RESP_METERED)) counted = 0;
   if (T.metrics && live && qos >= 0) {  // N3: the series the reference updates per response-body message
     unsigned long long* row = reinterpret_cast<unsigned long long*>(T.metrics + (size_t)qos * ARKS_METRIC_COLS);
     const uint8_t fl = B.flags[i];
@@ -1713,12 +1721,14 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32, ARKS_SSE_MINBLK) scan_sse
 // pass 1: one lane per body. Decoded `content` strings go to `text` (same offsets as the bodies), every pre-token becomes
 // a work-list entry: text offset | (length - 1) << 32 | body << 40. Entries are handed out 32 at a time (one atomic per flush).
 constexpr int kBpeFlush = 32;
+// Rows whose `row_flags` contain every bit of `wide_mask` count the wide key set (N5 metered rows); row_flags may be null.
 __global__ void __launch_bounds__(128) bpe_scan_kernel(const uint8_t* bodies, const uint32_t* body_off, const uint32_t* body_len, uint32_t n,
                                                        BpeTablesDev T, uint8_t* text, unsigned long long* list, uint32_t* list_n,
-                                                       uint32_t list_cap, uint32_t* bpe_out) {
+                                                       uint32_t list_cap, uint32_t* bpe_out, const uint8_t* row_flags, uint32_t wide_mask) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const uint32_t off = body_off[i];
+  const uint32_t keys = row_flags && (row_flags[i] & wide_mask) == wide_mask ? kBpeKeysWide : kBpeKeysContent;
   unsigned long long buf[kBpeFlush];
   uint32_t nb = 0, overflow = 0;
   auto flush = [&]() {
@@ -1729,7 +1739,7 @@ __global__ void __launch_bounds__(128) bpe_scan_kernel(const uint8_t* bodies, co
       for (uint32_t k = 0; k < nb; k++) list[at + k] = buf[k];
     nb = 0;
   };
-  const BpeScanOut o = bpe_scan_body(bodies + off, body_len[i], text + off, T, [&](uint32_t s, uint32_t len) {
+  const BpeScanOut o = bpe_scan_body(bodies + off, body_len[i], text + off, T, keys, [&](uint32_t s, uint32_t len) {
     buf[nb++] = (unsigned long long)(off + s) | (unsigned long long)(len - 1) << 32 | (unsigned long long)i << 40;
     if (nb == kBpeFlush) flush();
   });
@@ -1759,6 +1769,39 @@ __global__ void __launch_bounds__(kBpeMergeThreads) bpe_merge_kernel(const unsig
     const uint32_t ntok = bpe_piece_tokens(text + off, len, hot, T);
     atomicAdd(&bpe_out[body], ntok);
   }
+}
+
+// N5 (arks_set_stream_metering): bills the metered rows of a batch, one lane per row, after the BPE kernels. A row is metered
+// when it was answered ARKS_R_OK and its flags contain every bit of `mask`; it is billed its BPE count, or its body length
+// when there is no count (bpe null: no vocabulary; or ARKS_BPE_UNCOUNTED). qos: the current generation's index (response
+// rows were re-mapped at staging; -1 bills nothing). `side` 0: prompts (quota item prompt, gateway_token_usage{input}),
+// 1: completion chunks (quota item response, gateway_token_usage{output}); tpm / tpd and quota item total on both.
+__global__ void __launch_bounds__(128) meter_charge_kernel(DevTables T, uint32_t n, const uint8_t* reason, const uint8_t* flags, uint32_t mask,
+                                                           const int32_t* qos_of, const uint32_t* bpe, const uint32_t* body_len, int side) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  bool on = i < n && reason[i] == ARKS_R_OK && (flags[i] & mask) == mask;
+  const int32_t qos = on ? qos_of[i] : -1;
+  on = on && qos >= 0;
+  long long c = 0;
+  if (on) {
+    const uint32_t b = bpe ? bpe[i] : kBpeUncounted;
+    c = b == kBpeUncounted ? (long long)body_len[i] : (long long)b;
+  }
+  on = on && c != 0;
+  const QosAcct a = load_qos_acct(T, qos, on);
+  const uint32_t row = on ? (uint32_t)qos : 0u;
+#pragma unroll
+  for (int r = 0; r < 2; r++) warp_agg_add(T.rate + (size_t)(2 + r) * T.n_qos + row, c * (long long)a.nt[r], on && a.nt[r]);
+  const bool q_on = on && a.qt >= 0;
+  const size_t qrow = (size_t)(q_on ? a.qt : 0) * 3;
+  const long long add_side = c * (long long)a.nq[side], add_total = c * (long long)a.nq[2];
+  warp_agg_add(T.quota + qrow + side, add_side, q_on && add_side != 0);
+  warp_agg_add(T.quota + qrow + 2, add_total, q_on && add_total != 0);
+  if (T.qdelta) {  // quota shared across GPUs, as in account_usage
+    warp_agg_add(T.qdelta + qrow + side, add_side, q_on && add_side != 0);
+    warp_agg_add(T.qdelta + qrow + 2, add_total, q_on && add_total != 0);
+  }
+  if (T.metrics) warp_agg_add(T.metrics + (size_t)row * ARKS_METRIC_COLS + ARKS_METRIC_USAGE + side, c, on);
 }
 
 // syncQuotaUsage (arks_impl.go:226-296): one lane per ArksQuota, in place on the device copies of the CR status
@@ -1843,6 +1886,7 @@ struct arks_ctx {
   cudaStream_t cfg_stream = nullptr;  // config plane: the next generation's tables are uploaded here, off the data path
   std::mutex cfg_mu;                  // prepare (config thread) vs commit (batch thread)
   bool precharge = false;              // N4 (arks_set_precharge)
+  bool meter = false;                  // N5 (arks_set_stream_metering)
   bool split = false;                  // fast path: two lanes per document in pass A (fast_*_kernel2), ARKS_SPLIT=1; measured slower
   bool walk8 = true;                   // fast path, pass B: the step inlined eight times (true) or one copy in a loop
   int regroup = 1;                     // fast path: regroup a block's documents by structure between passes A and B
@@ -1896,6 +1940,7 @@ struct arks_ctx {
     RespDev rp{};
     uint32_t req_n = 0, resp_n = 0;
     int resp_mode = 0;  // 1 all JSON documents, 2 all SSE chunks, 0 mixed
+    bool resp_metered = false;  // the staged response batch has a metered chunk (N5): the meter kernel runs after the BPE kernels
     uint32_t resp_n_sse = 0;
     const uint32_t* d_resp_kind = nullptr;  // mixed batch: row indices, complete bodies first then SSE chunks
     bool req_staged = false, resp_staged = false;
@@ -1917,6 +1962,8 @@ struct arks_ctx {
   cudaEvent_t ev_bpe[2] = {nullptr, nullptr};   // around the two BPE kernels
   bool ev_bpe_set = false;
   cudaEvent_t ev_admit0 = nullptr;              // start of rank_hot + limit_admit (after the BPE kernels)
+  cudaEvent_t ev_meter[2] = {nullptr, nullptr}; // around meter_charge_kernel (N5)
+  bool ev_meter_set = false;
   bool is_req_timing = false;
   bool last_two_stage = false;
   const uint32_t* last_slow_n = nullptr;
@@ -2017,6 +2064,7 @@ int arks_create(int device, uint32_t max_batch, uint64_t max_batch_bytes, arks_c
   for (int k = 0; k < 4; k++) CK(cudaEventCreate(&ctx->ev[k]));
   for (int k = 0; k < 2; k++) CK(cudaEventCreate(&ctx->ev_fast[k]));
   for (int k = 0; k < 2; k++) CK(cudaEventCreate(&ctx->ev_bpe[k]));
+  for (int k = 0; k < 2; k++) CK(cudaEventCreate(&ctx->ev_meter[k]));
   CK(cudaEventCreate(&ctx->ev_admit0));
 #define ARKS_FOR_SCHED(X) X(0) X(1) X(8)
 #define ARKS_SET(S)                                                                                                        \
@@ -2110,6 +2158,7 @@ void arks_destroy(arks_ctx* ctx) {
   for (int k = 0; k < 2; k++) {
     if (ctx->ev_fast[k]) cudaEventDestroy(ctx->ev_fast[k]);
     if (ctx->ev_bpe[k]) cudaEventDestroy(ctx->ev_bpe[k]);
+    if (ctx->ev_meter[k]) cudaEventDestroy(ctx->ev_meter[k]);
   }
   if (ctx->ev_admit0) cudaEventDestroy(ctx->ev_admit0);
   cudaFree(ctx->d_inter);
@@ -2191,6 +2240,7 @@ void arks_free_pinned(void* p) {
 // ---- BPE side output ------------------------------------------------------------------------------
 int arks_load_bpe(arks_ctx* ctx, const arks_bpe_tables* t) {
   if (!ctx) return ARKS_E_INVALID_ARG;
+  if (!t && ctx->meter) return fail(ctx, ARKS_E_INVALID_ARG, "stream metering needs the vocabulary: switch it off first");
   CK(cudaSetDevice(ctx->device));
   CK(cudaStreamSynchronize(ctx->stream));
   for (void* p : ctx->bpe_allocs) cudaFree(p);
@@ -2229,14 +2279,25 @@ int arks_load_bpe(arks_ctx* ctx, const arks_bpe_tables* t) {
   ctx->bpe_on = true;
   return 0;
 }
-// queue the two BPE kernels for `n` bodies on the compute stream; counts land in bpe_out
-static int queue_bpe(arks_ctx* ctx, const uint8_t* bodies, const uint32_t* body_off, const uint32_t* body_len, uint32_t n, uint32_t* bpe_out) {
+// queue the two BPE kernels for `n` bodies on the compute stream; counts land in bpe_out. Rows whose row_flags (may be null)
+// contain every bit of wide_mask count the wide key set of metered rows
+static int queue_bpe(arks_ctx* ctx, const uint8_t* bodies, const uint32_t* body_off, const uint32_t* body_len, uint32_t n, uint32_t* bpe_out,
+                     const uint8_t* row_flags, uint32_t wide_mask) {
   CK(cudaMemsetAsync(ctx->d_bpe_n, 0, 4, ctx->stream));
   bpe_scan_kernel<<<(n + 127) / 128, 128, 0, ctx->stream>>>(bodies, body_off, body_len, n, ctx->bpe, ctx->d_bpe_text, ctx->d_bpe_list,
-                                                            ctx->d_bpe_n, ctx->bpe_list_cap, bpe_out);
+                                                            ctx->d_bpe_n, ctx->bpe_list_cap, bpe_out, row_flags, wide_mask);
   bpe_merge_kernel<<<ctx->n_sm * 4, kBpeMergeThreads, 0, ctx->stream>>>(ctx->d_bpe_list, ctx->d_bpe_n, ctx->bpe_list_cap, ctx->bpe,
                                                                         ctx->d_bpe_text, bpe_out);
   ctx->launches += 2;
+  return 0;
+}
+// queue meter_charge_kernel (N5) on the compute stream, timed on its own when profiling
+static int queue_meter(arks_ctx* ctx, uint32_t n, const uint8_t* reason, const uint8_t* flags, uint32_t mask, const int32_t* qos,
+                       const uint32_t* bpe, const uint32_t* body_len, int side) {
+  if (ctx->prof) CK(cudaEventRecord(ctx->ev_meter[0], ctx->stream));
+  meter_charge_kernel<<<(n + 127) / 128, 128, 0, ctx->stream>>>(ctx->dt, n, reason, flags, mask, qos, bpe, body_len, side);
+  if (ctx->prof) { CK(cudaEventRecord(ctx->ev_meter[1], ctx->stream)); ctx->ev_meter_set = true; }
+  ctx->launches += 1;
   return 0;
 }
 
@@ -2629,6 +2690,12 @@ int arks_set_precharge(arks_ctx* ctx, int on) {
   ctx->precharge = on != 0;
   return 0;
 }
+int arks_set_stream_metering(arks_ctx* ctx, int on) {
+  if (!ctx) return ARKS_E_INVALID_ARG;
+  if (on && !ctx->bpe_on) return fail(ctx, ARKS_E_NOT_LOADED, "stream metering needs a vocabulary (arks_load_bpe)");
+  ctx->meter = on != 0;
+  return 0;
+}
 
 int arks_update_endpoint_weights(arks_ctx* ctx, uint32_t ep, uint32_t n, const int32_t* w) {
   if (!ctx || !ctx->loaded) return ARKS_E_NOT_LOADED;
@@ -2705,7 +2772,8 @@ int arks_last_kernel_ms(arks_ctx* ctx, float* ms, int cap) {
   if (ctx->ev_n == 0) return 0;
   // request: scan stage, rank_hot + limit_admit, fast-path kernel alone (0 if not used), BPE kernels (0 if off)
   // response: scan stage, fast-path kernel alone, BPE kernels
-  float v[4] = {0, 0, 0, 0};
+  // both: + the meter kernel when it ran (N5)
+  float v[5] = {0, 0, 0, 0, 0};
   int n = 0;
   CK(cudaEventElapsedTime(&v[n++], ctx->ev[0], ctx->ev[1]));
   if (ctx->is_req_timing) CK(cudaEventElapsedTime(&v[n++], ctx->ev_admit0, ctx->ev[2]));
@@ -2713,6 +2781,7 @@ int arks_last_kernel_ms(arks_ctx* ctx, float* ms, int cap) {
   n++;
   if (ctx->ev_bpe_set) CK(cudaEventElapsedTime(&v[n], ctx->ev_bpe[0], ctx->ev_bpe[1]));
   n++;
+  if (ctx->ev_meter_set) CK(cudaEventElapsedTime(&v[n++], ctx->ev_meter[0], ctx->ev_meter[1]));
   for (int k = 0; k < n && k < cap; k++) ms[k] = v[k];
   return n < cap ? n : cap;
 }
@@ -2863,12 +2932,14 @@ int arks_run_request_batch(arks_ctx* ctx, int64_t now_unix) {
   ctx->ev_n = 0;
   ctx->ev_fast_set = false;
   ctx->ev_bpe_set = false;
+  ctx->ev_meter_set = false;
   ctx->last_two_stage = false;
   if (n == 0) return 0;
   CK(cudaStreamWaitEvent(ctx->stream, sl.req_copied, 0));
   ReqDev& r = sl.rq;
   sl.req_zc = n <= kZeroCopyRows && sl.h_req_result;
   carve_request(ctx, r, n, sl.req_zc ? sl.h_req_result : ctx->d_result);
+  r.meter = ctx->meter ? 1 : 0;
   // batch-local group table sized to the batch (2x, power of two); the three arrays are contiguous
   uint32_t g = 64;
   while (g < 2 * n) g <<= 1;
@@ -2929,7 +3000,7 @@ int arks_run_request_batch(arks_ctx* ctx, int64_t now_unix) {
   if (ctx->prof) CK(cudaEventRecord(ctx->ev[1], ctx->stream));
   if (ctx->bpe_on) {
     if (ctx->prof) CK(cudaEventRecord(ctx->ev_bpe[0], ctx->stream));
-    rc = queue_bpe(ctx, r.bodies, r.body_off, r.body_len, n, r.bpe);
+    rc = queue_bpe(ctx, r.bodies, r.body_off, r.body_len, n, r.bpe, ctx->meter ? r.st_flags : nullptr, ARKS_FLAG_METERED);
     if (rc) return rc;
     if (ctx->prof) { CK(cudaEventRecord(ctx->ev_bpe[1], ctx->stream)); ctx->ev_bpe_set = true; }
   }
@@ -2941,6 +3012,10 @@ int arks_run_request_batch(arks_ctx* ctx, int64_t now_unix) {
   r.precharge = ctx->precharge && ctx->bpe_on ? 1 : 0;
   limit_admit_kernel<<<(n + 127) / 128, 128, 0, ctx->stream>>>(ctx->dt, r);
   if (ctx->prof) { CK(cudaEventRecord(ctx->ev[2], ctx->stream)); ctx->ev_n = 3; ctx->is_req_timing = true; }
+  if (ctx->meter) {  // N5: the prompts of the admitted metered rows are charged when the micro-batch commits
+    rc = queue_meter(ctx, n, r.reason, r.flags, ARKS_FLAG_METERED, r.qos, ctx->bpe_on ? r.bpe : nullptr, r.body_len, 0);
+    if (rc) return rc;
+  }
   CK(cudaEventRecord(sl.req_ran, ctx->stream));
   ctx->launches += 2;
   CK(cudaGetLastError());
@@ -3051,14 +3126,16 @@ int arks_stage_response_batch(arks_ctx* ctx, const arks_response_batch* b) {
   sl.resp_n = n;
   if (n == 0) { sl.resp_staged = true; return 0; }
   if (!b->body_off || !b->body_len || !b->qos || !b->flags || (b->bodies_bytes && !b->bodies)) return fail(ctx, ARKS_E_INVALID_ARG, "response batch: null array");
-  uint32_t n_sse = 0;
+  uint32_t n_sse = 0, n_metered = 0;
   for (uint32_t i = 0; i < n; i++) {
     n_sse += (b->flags[i] & ARKS_RESP_STREAM) != 0;
+    n_metered += (b->flags[i] & (ARKS_RESP_STREAM | ARKS_RESP_METERED)) == (ARKS_RESP_STREAM | ARKS_RESP_METERED);
     if ((b->body_off[i] & 15u) || (uint64_t)b->body_off[i] + b->body_len[i] > b->bodies_bytes)
       return fail(ctx, ARKS_E_INVALID_ARG, "body %u: offset not 16-byte aligned or out of range", i);
   }
   sl.resp_mode = n_sse == 0 ? 1 : n_sse == n ? 2 : 0;
   sl.resp_n_sse = n_sse;
+  sl.resp_metered = n_metered != 0;
   size_t o_off = 0, o_len = align_up((size_t)n * 4, 256), o_qos = o_len * 2, o_fl = o_len * 3, o_kind = o_fl + align_up(n, 256),
          o_pre = o_kind + (sl.resp_mode == 0 ? o_len : 0), total = o_pre + (b->precharged ? o_len : 0);
   if (total + (b->bodies_bytes <= kTinyBatchBytes ? b->bodies_bytes : 0) > ctx->meta_cap) return fail(ctx, ARKS_E_CAPACITY, "response metadata exceeds capacity");
@@ -3128,6 +3205,7 @@ int arks_run_response_batch(arks_ctx* ctx, int64_t now_unix) {
   ctx->ev_n = 0;
   ctx->ev_fast_set = false;
   ctx->ev_bpe_set = false;
+  ctx->ev_meter_set = false;
   ctx->last_two_stage = false;
   if (n == 0) return 0;
   const uint32_t tpb = kWarpsPerBlock * 32;
@@ -3215,11 +3293,17 @@ int arks_run_response_batch(arks_ctx* ctx, int64_t now_unix) {
   if (ctx->prof) { CK(cudaEventRecord(ctx->ev[1], ctx->stream)); ctx->ev_n = 2; ctx->is_req_timing = false; }
   if (ctx->bpe_on) {
     if (ctx->prof) CK(cudaEventRecord(ctx->ev_bpe[0], ctx->stream));
-    rc = queue_bpe(ctx, sl.rp.bodies, sl.rp.body_off, sl.rp.body_len, n, sl.rp.bpe);
+    rc = queue_bpe(ctx, sl.rp.bodies, sl.rp.body_off, sl.rp.body_len, n, sl.rp.bpe, sl.resp_metered ? sl.rp.flags : nullptr,
+                   ARKS_RESP_STREAM | ARKS_RESP_METERED);
     if (rc) return rc;
     if (ctx->prof) { CK(cudaEventRecord(ctx->ev_bpe[1], ctx->stream)); ctx->ev_bpe_set = true; }
   } else {
     CK(cudaMemsetAsync(sl.rp.bpe, 0, (size_t)n * 4, ctx->stream));
+  }
+  if (sl.resp_metered) {  // N5: metered chunks answered ARKS_R_OK are billed their completion count
+    rc = queue_meter(ctx, n, sl.rp.reason, sl.rp.flags, ARKS_RESP_STREAM | ARKS_RESP_METERED, sl.rp.qos, ctx->bpe_on ? sl.rp.bpe : nullptr,
+                     sl.rp.body_len, 1);
+    if (rc) return rc;
   }
   CK(cudaEventRecord(sl.resp_ran, ctx->stream));
   ctx->launches += 1;

@@ -5,7 +5,8 @@
 // unless the host opts in, and its oracle is HF `tokenizers` (tests/test_bpe.py), not the Go code.
 //
 //   what is counted   every JSON string that is the value of a key named `content` (the messages of a chat request, the
-//                     message / delta of a completion or SSE chunk), escapes decoded
+//                     message / delta of a completion or SSE chunk), escapes decoded; on metered rows (N5,
+//                     arks_set_stream_metering) also `text`, `reasoning_content` and `arguments`
 //   pass 1  (bpe_scan_body, one lane per body)  a byte scanner finds those strings, decodes them into a scratch text
 //           buffer and cuts them into pieces with the Qwen2 pre-tokenizer pattern
 //           (transformers/models/qwen2/tokenization_qwen2.py:33) written out as a hand scanner over Unicode classes
@@ -208,25 +209,54 @@ ARKS_HD void bpe_pretokenize(const uint8_t* t, uint32_t s, uint32_t e, const uin
   }
 }
 
+// ---- key sets: the names whose string values are counted. Bit k selects name k; all candidates are matched at once ----
+constexpr uint32_t kBpeKeysContent = 1u;  // `content` only: every row that is not metered
+constexpr uint32_t kBpeKeysWide = 15u;    // + `text` (content parts), `reasoning_content`, `arguments` (tool calls): metered rows
+// The names are packed little-endian into 64-bit immediates (no loads, no pointers held in registers); bytes past a name
+// are 0. A candidate that survives past its length is harmless: bpe_key_done wants the exact length.
+ARKS_HD constexpr uint64_t bpe_pack8(const char* s, uint32_t n) {
+  uint64_t v = 0;
+  for (uint32_t i = n; i-- > 0;) v = v << 8 | (uint8_t)s[i];
+  return v;
+}
+constexpr uint64_t kKeyContent = bpe_pack8("content", 7), kKeyText = bpe_pack8("text", 4);
+constexpr uint64_t kKeyReason0 = bpe_pack8("reasoning_content", 8), kKeyReason1 = bpe_pack8("reasoning_content" + 8, 8), kKeyReason2 = 't';
+constexpr uint64_t kKeyArgs0 = bpe_pack8("arguments", 8), kKeyArgs1 = 's';
+// candidates still equal to the decoded key after its character `cp` at position `pos`
+ARKS_HD uint32_t bpe_key_step(uint32_t cand, uint32_t pos, uint32_t cp) {
+  if (cp >= 0x80 || pos >= 17) return 0;
+  const uint32_t sh = 8 * (pos & 7);
+  const bool lo = pos < 8, mid = pos >= 8 && pos < 16;
+  const uint32_t c0 = lo ? (uint32_t)(kKeyContent >> sh) & 0xffu : 0u;
+  const uint32_t c1 = lo ? (uint32_t)(kKeyText >> sh) & 0xffu : 0u;
+  const uint32_t c2 = (uint32_t)((lo ? kKeyReason0 : mid ? kKeyReason1 : kKeyReason2) >> sh) & 0xffu;
+  const uint32_t c3 = (uint32_t)((lo ? kKeyArgs0 : mid ? kKeyArgs1 : 0ull) >> sh) & 0xffu;
+  return cand & ((c0 == cp ? 1u : 0u) | (c1 == cp ? 2u : 0u) | (c2 == cp ? 4u : 0u) | (c3 == cp ? 8u : 0u));
+}
+// a candidate of exactly `pos` characters is left
+ARKS_HD bool bpe_key_done(uint32_t cand, uint32_t pos) {
+  return ((cand & 1u) && pos == 7) || ((cand & 2u) && pos == 4) || ((cand & 4u) && pos == 17) || ((cand & 8u) && pos == 9);
+}
+
 // ---- pass 1: one body ----
 struct BpeScanOut {
   uint32_t pieces;  // emitted
   uint32_t bad;     // the body is reported as uncounted
 };
-// text: scratch for the decoded strings of this body (capacity >= len bytes). emit(text offset, length) per piece.
+// text: scratch for the decoded strings of this body (capacity >= len bytes). keys: kBpeKeysContent or kBpeKeysWide.
+// emit(text offset, length) per piece.
 template <class E>
-ARKS_HD BpeScanOut bpe_scan_body(const uint8_t* b, uint32_t len, uint8_t* text, const BpeTablesDev& T, E&& emit) {
+ARKS_HD BpeScanOut bpe_scan_body(const uint8_t* b, uint32_t len, uint8_t* text, const BpeTablesDev& T, uint32_t keys, E&& emit) {
   BpeScanOut o{0, 0};
   uint32_t i = 0, wr = 0;
-  bool last_string = false, last_is_content = false, expect = false;
-  const char* kContent = "content";
+  bool last_string = false, last_is_key = false, expect = false;
   while (i < len && !o.bad) {
     const uint8_t c = b[i];
     if (c == '"') {
       const bool count_it = expect;
       expect = false;
       const uint32_t w0 = wr;
-      uint32_t match = 0;  // decoded bytes equal to "content" so far; 0xFF: differs
+      uint32_t cand = keys, pos = 0;  // key names still equal to the decoded string, its decoded length
       bool closed = false, unsafe = false;
       i++;
       while (i < len) {
@@ -271,7 +301,8 @@ ARKS_HD BpeScanOut bpe_scan_body(const uint8_t* b, uint32_t len, uint8_t* text, 
           i += need;
         }
         if (bpe_class(T.cp_class, cp) & UC_NFC_UNSAFE) unsafe = true;
-        if (match != 0xFF) match = (cp < 0x80 && match < 7 && (uint8_t)kContent[match] == cp) ? match + 1 : 0xFF;
+        if (cand) cand = bpe_key_step(cand, pos, cp);
+        pos++;
         wr += bpe_put_utf8(text, wr, cp);
       }
       if (!closed) { o.bad = 1; break; }
@@ -285,16 +316,20 @@ ARKS_HD BpeScanOut bpe_scan_body(const uint8_t* b, uint32_t len, uint8_t* text, 
         wr = w0;  // not counted: the scratch is reused
       }
       last_string = true;
-      last_is_content = match == 7;
+      last_is_key = bpe_key_done(cand, pos);
       continue;
     }
     if (c == ' ' || c == '\t' || c == '\n' || c == '\r') { i++; continue; }
-    if (c == ':' && last_string && last_is_content) expect = true;
+    if (c == ':' && last_string && last_is_key) expect = true;
     else expect = false;
     last_string = false;
     i++;
   }
   return o;
+}
+template <class E>
+ARKS_HD BpeScanOut bpe_scan_body(const uint8_t* b, uint32_t len, uint8_t* text, const BpeTablesDev& T, E&& emit) {
+  return bpe_scan_body(b, len, text, T, kBpeKeysContent, emit);
 }
 
 // ---- host: the merge list as the two hash tables the lookups use (also used by the CPU test build) ----

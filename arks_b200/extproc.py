@@ -507,7 +507,9 @@ class ExtProcServer:
         r = PB["ProcessingResponse"]()
         r.request_body.response.header_mutation.CopyFrom(_set_headers([
             ("model", t.qos_model_name[q]), ("namespace", t.token_namespace[tok]), ("username", t.token_user[tok])]))
-        return r, (q, out.get("gen")), bool(out["flags"] & 1)
+        # a stream's response flags: RESP_METERED rides on every chunk of a stream admitted with FLAG_METERED (N5)
+        fl = int(out["flags"])
+        return r, (q, out.get("gen")), (abi.RESP_STREAM | (abi.RESP_METERED if fl & abi.FLAG_METERED else 0)) if fl & 1 else 0
 
     # ---- HandleResponseHeaders, handle_response.go:37-78
     def handle_response_headers(self, req):
@@ -527,10 +529,11 @@ class ExtProcServer:
 
     # ---- HandleResponseBody, handle_response.go:80-268
     def handle_response_body(self, req, qos, stream, buffered):
+        """`stream`: 0, or the RESP_* flags of the stream's chunks (handle_request_body)"""
         body, eos = bytes(req.response_body.body), req.response_body.end_of_stream
         qos, gen = qos
         if stream:
-            out = self.batcher.response(body, qos, abi.RESP_STREAM, gen)
+            out = self.batcher.response(body, qos, stream, gen)
         else:
             buffered += body  # requestBuffers, handle_response.go:134-155
             if not eos:

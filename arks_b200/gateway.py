@@ -64,6 +64,7 @@ def lib():
         L.arks_find_qos.argtypes = [vp, cp, u32, cp, u32, cp, u32]
         L.arks_find_qos.restype = C.c_int32
         L.arks_set_precharge.argtypes = [vp, C.c_int]
+        L.arks_set_stream_metering.argtypes = [vp, C.c_int]
         L.arks_table_generation.restype = C.c_uint32
         L.arks_table_generation.argtypes = [vp]
         L.arks_update_endpoint_weights.argtypes = [vp, C.c_uint32, C.c_uint32, abi.i32p]
@@ -113,6 +114,7 @@ def lib():
 
 EXPORTED = [  # every symbol include/arks_gateway.h declares (checked by tests/test_abi.py)
     "arks_abi_version", "arks_create", "arks_destroy", "arks_last_error", "arks_load_tables", "arks_table_generation", "arks_load_bpe", "arks_set_precharge",
+    "arks_set_stream_metering",
     "arks_prepare_tables", "arks_commit_tables", "arks_discard_prepared", "arks_upsert_token", "arks_delete_token", "arks_upsert_quota",
     "arks_delete_quota", "arks_upsert_endpoint", "arks_delete_endpoint", "arks_config_prepare", "arks_find_quota", "arks_find_qos",
     "arks_update_endpoint_weights", "arks_extract_bearer", "arks_submit_request_batch",
@@ -239,6 +241,12 @@ class Gateway:
         carry `precharged` reconcile (needs load_bpe; changes admit / deny against the reference)"""
         self._ck(lib().arks_set_precharge(self._h, int(bool(on))))
 
+    def set_stream_metering(self, on: bool):
+        """N5, opt-in: stream requests without stream_options.include_usage are decided instead of refused and billed by their
+        BPE counts (result flags & abi.FLAG_METERED; the host must set abi.RESP_METERED on every chunk of such a stream).
+        Needs load_bpe"""
+        self._ck(lib().arks_set_stream_metering(self._h, int(bool(on))))
+
     @property
     def generation(self) -> int:
         """table generation the qos / token indices of request results refer to (carry it with the stream)"""
@@ -316,9 +324,9 @@ class Gateway:
 
     def last_kernel_ms(self):
         """request batch: [scan stage, rank + admit, fast-path kernel alone or 0, BPE kernels or 0]; response batch: the
-        same without the admit entry"""
-        buf = (C.c_float * 4)()
-        n = lib().arks_last_kernel_ms(self._h, buf, 4)
+        same without the admit entry; both + [meter kernel] when it ran (N5)"""
+        buf = (C.c_float * 5)()
+        n = lib().arks_last_kernel_ms(self._h, buf, 5)
         if n < 0:
             self._ck(n)
         return [float(buf[k]) for k in range(n)]

@@ -1029,6 +1029,7 @@ Action StreamProcessor::OnRequestBody(std::string_view body, uint64_t pick_rand)
   qos_ = req_.qos;
   gen_ = req_.gen;
   stream_ = req_.flags & 1;
+  metered_ = (req_.flags & ARKS_FLAG_METERED) != 0;
   Action a;
   a.kind = Action::kContinueRequestBody;
   a.set_headers.push_back({"model", nm->qos_model[(size_t)req_.qos]});
@@ -1058,7 +1059,7 @@ Action StreamProcessor::OnResponseBody(std::string_view body, bool end_of_stream
   // gateway.go:122-126: the upstream's error body is passed on; `resp` is still empty there, so no x-error-* header
   if (status_ != 200) return ErrorResponse(status_, {}, std::string(body));
   if (stream_) {
-    resp_ = b_->HandleResponseBody(qos_, gen_, body, ARKS_RESP_STREAM, Estimate());
+    resp_ = b_->HandleResponseBody(qos_, gen_, body, ARKS_RESP_STREAM | (metered_ ? ARKS_RESP_METERED : 0u), Estimate());
   } else {
     buffered_.append(body);  // requestBuffers, handle_response.go:134-155
     if (!end_of_stream) {

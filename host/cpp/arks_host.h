@@ -182,6 +182,9 @@ class StreamProcessor {
   int32_t qos_ = -1;
   uint32_t gen_ = 0;
   bool stream_ = false;
+  // the request was admitted with ARKS_FLAG_METERED (N5, arks_set_stream_metering on the Batcher's context): every chunk
+  // carries ARKS_RESP_METERED
+  bool metered_ = false;
   int status_ = 0;
   RequestDecision req_{};
   ResponseDecision resp_{};

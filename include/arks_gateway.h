@@ -162,7 +162,7 @@ typedef struct arks_request_batch {
 typedef struct arks_request_result {
   uint8_t* reason;      /* n: enum arks_reason; ARKS_R_OK == continue (BodyResponse + 3 headers)            */
   uint8_t* detail;      /* n: rule / quota-item index for 429s, else 0                                       */
-  uint8_t* flags;       /* n: bit0 = stream                                                                  */
+  uint8_t* flags;       /* n: bit0 = stream, bit1 = ARKS_FLAG_METERED                                        */
   int32_t* qos;         /* n: qos-entry index carried into the response phase, -1 if not resolved            */
   int32_t* token;       /* n: ArksToken index (namespace / username headers), -1 if not found                */
   int32_t* pick;        /* n: backend index within the endpoint, -1 none / not admitted                      */
@@ -178,6 +178,7 @@ typedef struct arks_request_result {
                          *    output: the reference counts no tokens at request time (check.go:124-126), so this never
                          *    feeds admit/deny unless arks_set_precharge is switched on                              */
 } arks_request_result;
+#define ARKS_FLAG_METERED 2u /* admitted under arks_set_stream_metering: the host sets ARKS_RESP_METERED on every chunk */
 
 /* ---- response phase (ProcessingRequest_ResponseBody with :status 200, handle_response.go:80-268) ---- */
 #define ARKS_RESP_STREAM 1u        /* the request had stream:true  -> body is one SSE chunk, decoded in isolation */
@@ -185,6 +186,8 @@ typedef struct arks_request_result {
                                     * chunk (only the metrics read it there)                                      */
 #define ARKS_RESP_COMPLETED 4u     /* this stream already had a usage-bearing message (`completed`, gateway.go:127):
                                     * read by the metrics only                                                     */
+#define ARKS_RESP_METERED 8u       /* with ARKS_RESP_STREAM: a chunk of a stream whose request result had ARKS_FLAG_METERED.
+                                    * Billed by its BPE count (arks_set_stream_metering); ignored on non-stream rows */
 typedef struct arks_response_batch {
   uint32_t n;
   const uint8_t* bodies;
@@ -298,6 +301,23 @@ int arks_load_bpe(arks_ctx* ctx, const arks_bpe_tables* t);
  * arks_response_batch.precharged. A stream whose response never arrives keeps its estimate charged. Quotas are untouched
  * (they bill what the upstream reports). Off by default: decisions are the reference's. */
 int arks_set_precharge(arks_ctx* ctx, int on);
+/* N5, OPT-IN stream metering. The reference refuses every stream:true request without stream_options.include_usage:true
+ * (ARKS_R_STREAM_OPTIONS, handle_request.go:156-171) because it cannot bill such a stream. With metering on such a request
+ * is decided like any other (rate limits, then quota); if admitted its result row has ARKS_FLAG_METERED and the host must
+ * set ARKS_RESP_METERED on every response chunk of that stream. Billing of a metered stream:
+ *   - its prompt's BPE count when its micro-batch commits: count x (tpm entries) and x (tpd entries) on the rate counters,
+ *     quota items prompt and total, gateway_token_usage{input};
+ *   - every chunk answered ARKS_R_OK: its completion count on tpm / tpd, quota items response and total,
+ *     gateway_token_usage{output}. An upstream `usage` in the chunk is still reported but NOT billed (counted = 0);
+ *   - a count that is not available (ARKS_BPE_UNCOUNTED, no vocabulary) is replaced by the body's byte length, an upper
+ *     bound of its byte-level BPE count;
+ *   - the pre-charge (arks_set_precharge) skips metered rows and their `precharged` is ignored: billed exactly once.
+ * Metered rows count every JSON string that is the value of a key named content, text, reasoning_content or arguments
+ * (bpe_count reports that wider count for every stream:true request without include_usage while metering is on, admitted
+ * or not, and for ARKS_RESP_METERED chunks; other rows keep the content-only count). Known under-counts: tool
+ * definitions, chat-template tokens. Needs a vocabulary: ARKS_E_NOT_LOADED without one, and arks_load_bpe(NULL) is refused
+ * while metering is on. Off by default: decisions are the reference's. */
+int arks_set_stream_metering(arks_ctx* ctx, int on);
 
 /* routing churn (BASELINE config 5): replace the weights of one endpoint's backends in place */
 int arks_update_endpoint_weights(arks_ctx* ctx, uint32_t endpoint, uint32_t n, const int32_t* weights);
