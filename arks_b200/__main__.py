@@ -40,7 +40,58 @@ def parse_args(argv=None):
     p.add_argument("--max-batch-bytes", dest="max_bytes", type=int, default=64 << 20)
     p.add_argument("--batcher", choices=("compiled", "python"), default="compiled", help="the C++ micro-batcher or its Python twin")
     p.add_argument("--grpc-workers", dest="workers", type=int, default=256, help="concurrent ext_proc streams served")
+    p.add_argument("--bpe.tokenizer", dest="bpe_tokenizer", default=None,
+                   help="tokenizer.json every model's text is BPE-counted with unless bound to another (off by default)")
+    p.add_argument("--bpe.model-tokenizer", dest="bpe_model_tokenizer", action="append", default=[], metavar="MODEL=PATH",
+                   help="count MODEL (an ArksEndpoint name) with the tokenizer.json at PATH; repeatable, the same PATH shares one "
+                        "vocabulary; needs --bpe.tokenizer")
+    p.add_argument("--bpe.precharge", dest="bpe_precharge", action="store_true",
+                   help="charge admitted requests' BPE counts to tpm / tpd at request time (needs --bpe.tokenizer)")
+    p.add_argument("--bpe.stream-metering", dest="bpe_stream_metering", action="store_true",
+                   help="decide and bill streams without stream_options.include_usage by their BPE counts (needs --bpe.tokenizer)")
     return p.parse_args(argv)
+
+
+def configure_bpe(engine, args, load=None):
+    """The --bpe.* flags as library calls, made before the first generation is published so that its tables already carry
+    the bindings: the default vocabulary into slot 0, every other tokenizer file into a slot of its own (models naming the
+    same file share it), one binding per model, then the pre-charge and stream metering switches. Without the flags: no
+    call at all. ValueError on flags that cannot work together."""
+    from . import bpe
+    load = load or bpe.load_tokenizer
+    a = args
+    pairs = []
+    for spec in a.bpe_model_tokenizer:
+        model, eq, path = spec.partition("=")
+        if not eq or not model or not path:
+            raise ValueError(f"--bpe.model-tokenizer {spec!r}: expected MODEL=PATH")
+        pairs.append((model, path))
+    if not a.bpe_tokenizer:
+        if pairs or a.bpe_precharge or a.bpe_stream_metering:
+            raise ValueError("--bpe.model-tokenizer, --bpe.precharge and --bpe.stream-metering need --bpe.tokenizer")
+        return
+    # one slot per FILE: two spellings of the same path (relative / absolute, a symlink) share it
+    key = os.path.realpath
+    slot_of, first_path = {key(a.bpe_tokenizer): 0}, [a.bpe_tokenizer]
+    for _, path in pairs:
+        if key(path) not in slot_of:
+            slot_of[key(path)] = len(first_path)
+            first_path.append(path)
+    if len(first_path) > bpe.MAX_VOCABS:
+        raise ValueError(f"{len(first_path)} tokenizer files: at most {bpe.MAX_VOCABS} vocabularies")
+    for slot, path in enumerate(first_path):
+        t = load(path)
+        if slot == 0 and not t.flags & bpe.BPE_IGNORE_MERGES:
+            engine.load_bpe(t)
+        else:
+            engine.load_bpe_vocab(slot, t)
+    for model, path in pairs:
+        if slot_of[key(path)]:
+            engine.bind_model_vocab(model, slot_of[key(path)])
+    if a.bpe_precharge:
+        engine.set_precharge(True)
+    if a.bpe_stream_metering:
+        engine.set_stream_metering(True)
 
 
 def read_objects(path):
@@ -163,6 +214,7 @@ def main(argv=None) -> int:
     from .gateway import Gateway
     g = Gateway(args.device, args.max_batch, args.max_bytes)  # raises without a CUDA device
     g.enable_metrics(True)
+    configure_bpe(g, args)  # before Assembly.start() publishes the first generation
     batcher = None
     if args.batcher == "compiled":
         batcher = extproc.CompiledBatcher(cpphost.Batcher(cpphost.load(cpphost.build()), g._h, max_batch=args.max_batch,

@@ -4,7 +4,9 @@
   load_tokenizer(path or dict)   HF tokenizer.json (or vocab.json + merges.txt) -> BpeTables, the flat arrays arks_load_bpe
                                  takes: the id of every single-byte token, the merge list (rank = index) as id triples, the
                                  Unicode class table of the Qwen2 split pattern (arks_b200/data/bpe_unicode.bin.z) and
-                                 whether the tokenizer normalises to NFC
+                                 the flags: NFC normalisation, the Llama 3 number split, `ignore_merges` (then also the
+                                 vocabulary's token strings, which arks_load_bpe_vocab takes). Only the Qwen2 and Llama 3
+                                 families are accepted; anything else raises ValueError instead of being miscounted
   content_strings(body)          what is counted: every string that is the value of a key named `content` (the messages of
                                  a chat request, the message / delta of a completion), JSON escapes decoded; with
                                  keys=METERED_KEYS the wider set metered streams count (N5, arks_set_stream_metering)
@@ -30,7 +32,13 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 UNICODE_TABLE = os.path.join(HERE, "data", "bpe_unicode.bin.z")
 QWEN2_PATTERN = (r"""(?i:'s|'t|'re|'ve|'m|'ll|'d)|[^\r\n\p{L}\p{N}]?\p{L}+|\p{N}| ?[^\s\p{L}\p{N}]+[\r\n]*|\s*[\r\n]+"""
                  r"""|\s+(?!\S)|\s+""")
+# Llama 3: the same alternatives, but numbers in runs of up to three
+LLAMA3_PATTERN = QWEN2_PATTERN.replace(r"|\p{N}|", r"|\p{N}{1,3}|")
 BPE_NFC = 1            # arks_bpe_tables.flags
+BPE_DIGITS3 = 2        # the pre-tokenizer splits numbers as \p{N}{1,3} (LLAMA3_PATTERN)
+BPE_IGNORE_MERGES = 4  # a pre-token that is a vocabulary entry is one token (the BPE model's "ignore_merges": true)
+MAX_VOCABS = 8         # ARKS_BPE_MAX_VOCABS
+MAX_PIECE = 128        # bytes of one pre-token the device counts (kBpeMaxPiece)
 UNCOUNTED = 0xFFFFFFFF  # ARKS_BPE_UNCOUNTED
 CONTENT_KEYS = ("content",)
 # metered rows (N5): also content parts ({"type":"text","text":..}), reasoning streams and tool-call arguments
@@ -64,6 +72,9 @@ class BpeTables:
     merged: np.ndarray
     cp_class: np.ndarray  # [0x110000 / 2] uint8, a nibble per code point (tools/gen_bpe_unicode.py)
     flags: int
+    # BPE_IGNORE_MERGES only: the token strings of 2..MAX_PIECE bytes, token k = tok_bytes[tok_off[k]:tok_off[k + 1]]
+    tok_bytes: np.ndarray | None = None  # uint8
+    tok_off: np.ndarray | None = None    # [n + 1] uint32
 
     def c_struct(self) -> ArksBpeTables:
         p32 = lambda a: a.ctypes.data_as(C.POINTER(C.c_uint32))
@@ -75,12 +86,46 @@ def unicode_classes() -> np.ndarray:
     return np.frombuffer(zlib.decompress(open(UNICODE_TABLE, "rb").read()), np.uint8).copy()
 
 
+def _check_tokenizer_json(tj) -> int:
+    """the flags of a tokenizer.json this counter reproduces exactly, or ValueError naming what it does not"""
+    model = tj.get("model") or {}
+    if model.get("type") != "BPE":
+        raise ValueError(f"unsupported model type {model.get('type')!r}: only byte-level BPE")
+    if model.get("dropout") not in (None, 0, 0.0):
+        raise ValueError("unsupported BPE dropout")
+    if model.get("byte_fallback"):
+        raise ValueError("unsupported byte_fallback (SentencePiece-style BPE)")
+    for k in ("continuing_subword_prefix", "end_of_word_suffix"):
+        if model.get(k):
+            raise ValueError(f"unsupported {k} {model[k]!r}")
+    norm = tj.get("normalizer")
+    if norm is not None and norm.get("type") != "NFC":
+        raise ValueError(f"unsupported normalizer {norm.get('type')!r}: only none or NFC")
+    pre = tj.get("pre_tokenizer") or {}
+    seq = pre.get("pretokenizers") if pre.get("type") == "Sequence" else None
+    if not seq or len(seq) != 2 or seq[0].get("type") != "Split" or seq[1].get("type") != "ByteLevel":
+        raise ValueError(f"unsupported pre-tokenizer {json.dumps(pre)[:200]}: only Sequence[Split(regex), ByteLevel(use_regex=false)]")
+    split, bl = seq
+    regex = (split.get("pattern") or {}).get("Regex")
+    if regex not in (QWEN2_PATTERN, LLAMA3_PATTERN):
+        raise ValueError(f"unsupported split pattern {json.dumps(split.get('pattern'))[:200]}: only the Qwen2 and Llama 3 patterns")
+    if split.get("behavior") != "Isolated" or split.get("invert"):
+        raise ValueError(f"unsupported split behaviour {split.get('behavior')!r} invert={split.get('invert')!r}")
+    if bl.get("use_regex", True):
+        raise ValueError("unsupported ByteLevel(use_regex=true): the GPT-2 pre-tokenizer")
+    if bl.get("add_prefix_space"):
+        raise ValueError("unsupported ByteLevel(add_prefix_space=true)")
+    return ((BPE_NFC if norm is not None else 0) | (BPE_DIGITS3 if regex == LLAMA3_PATTERN else 0)
+            | (BPE_IGNORE_MERGES if model.get("ignore_merges") else 0))
+
+
 def load_tokenizer(src, merges_txt: str | None = None) -> BpeTables:
-    """src: path of a tokenizer.json / its parsed dict / its JSON text, or the path of a vocab.json when merges_txt is given"""
+    """src: path of a tokenizer.json / its parsed dict / its JSON text, or the path of a vocab.json when merges_txt is given
+    (a Qwen2 vocabulary). A tokenizer.json must be a Qwen2 or Llama 3 style byte-level BPE (_check_tokenizer_json)."""
     if merges_txt is not None:
         vocab = json.load(open(src))
         merges = [tuple(l.split(" ")) for l in open(merges_txt).read().split("\n") if l and not l.startswith("#version")]
-        normalizer = None
+        flags = 0
     else:
         if isinstance(src, dict):
             tj = src
@@ -88,11 +133,9 @@ def load_tokenizer(src, merges_txt: str | None = None) -> BpeTables:
             tj = json.loads(src)
         else:
             tj = json.load(open(src))
-        if tj["model"]["type"] != "BPE":
-            raise ValueError("only byte-level BPE tokenizers are supported")
+        flags = _check_tokenizer_json(tj)
         vocab = tj["model"]["vocab"]
         merges = [tuple(m) if isinstance(m, list) else tuple(m.split(" ")) for m in tj["model"]["merges"]]
-        normalizer = tj.get("normalizer")
     b2u = bytes_to_unicode()
     byte_id = np.zeros(256, np.uint32)
     for b in range(256):
@@ -102,9 +145,18 @@ def load_tokenizer(src, merges_txt: str | None = None) -> BpeTables:
     left = np.fromiter((vocab[a] for a, _ in merges), np.uint32, len(merges))
     right = np.fromiter((vocab[b] for _, b in merges), np.uint32, len(merges))
     merged = np.fromiter((vocab[a + b] for a, b in merges), np.uint32, len(merges))
-    flags = BPE_NFC if normalizer and (normalizer.get("type") == "NFC" or any(
-        n.get("type") == "NFC" for n in normalizer.get("normalizers", []))) else 0
-    return BpeTables(byte_id, left, right, merged, unicode_classes(), flags)
+    t = BpeTables(byte_id, left, right, merged, unicode_classes(), flags)
+    if flags & BPE_IGNORE_MERGES:
+        # a pre-token is looked up as its byte-level string; entries with a character outside that alphabet never match
+        u2b = {u: b for b, u in bytes_to_unicode().items()}
+        strs = []
+        for s in vocab:
+            if 2 <= len(s) <= MAX_PIECE and all(c in u2b for c in s):
+                strs.append(bytes(u2b[c] for c in s))
+        t.tok_off = np.zeros(len(strs) + 1, np.uint32)
+        t.tok_off[1:] = np.cumsum([len(x) for x in strs], dtype=np.uint64).astype(np.uint32)
+        t.tok_bytes = np.frombuffer(b"".join(strs), np.uint8).copy()
+    return t
 
 
 def content_strings(body: bytes, keys=CONTENT_KEYS) -> list[str]:
@@ -160,16 +212,21 @@ def _corpus(n_lines: int, seed: int):
         yield " ".join(toks)
 
 
-def standin_tokenizer(vocab_size: int = 151_643, seed: int = 0xB9E, cache_dir: str | None = None):
-    """-> (tokenizers.Tokenizer, tokenizer.json text). Deterministic; cached under cache_dir when given."""
+def standin_tokenizer(vocab_size: int = 151_643, seed: int = 0xB9E, cache_dir: str | None = None, pattern: str = QWEN2_PATTERN,
+                      ignore_merges: bool = False):
+    """-> (tokenizers.Tokenizer, tokenizer.json text). Deterministic; cached under cache_dir when given. pattern=LLAMA3_PATTERN,
+    ignore_merges=True: a Llama 3 style stand-in (with the defaults, the Qwen2 one, unchanged)."""
     from tokenizers import Regex, Tokenizer, decoders, models, pre_tokenizers, trainers
-    path = os.path.join(cache_dir, f"standin_bpe_{vocab_size}_{seed:x}.json") if cache_dir else None
+    if pattern not in (QWEN2_PATTERN, LLAMA3_PATTERN):
+        raise ValueError("pattern: QWEN2_PATTERN or LLAMA3_PATTERN")
+    variant = ("_llama3" if pattern == LLAMA3_PATTERN else "") + ("_im" if ignore_merges else "")
+    path = os.path.join(cache_dir, f"standin_bpe_{vocab_size}_{seed:x}{variant}.json") if cache_dir else None
     if path and os.path.exists(path):
         text = open(path).read()
         return Tokenizer.from_str(text), text
-    tok = Tokenizer(models.BPE())
+    tok = Tokenizer(models.BPE(ignore_merges=True) if ignore_merges else models.BPE())
     tok.pre_tokenizer = pre_tokenizers.Sequence([
-        pre_tokenizers.Split(Regex(QWEN2_PATTERN), behavior="isolated", invert=False),
+        pre_tokenizers.Split(Regex(pattern), behavior="isolated", invert=False),
         pre_tokenizers.ByteLevel(add_prefix_space=False, use_regex=False)])
     tok.decoder = decoders.ByteLevel()
     trainer = trainers.BpeTrainer(vocab_size=vocab_size, special_tokens=[], show_progress=False,

@@ -78,6 +78,7 @@ struct DevTables {
   const uint32_t* qos_model_len;
   const int32_t* qos_quota;
   const int32_t* qos_ep;  // endpoint index for (token namespace, model) or -1
+  const uint8_t* qos_vocab;  // BPE vocabulary slot of the entry's model (arks_bind_model_vocab; 0: the default)
   const uint32_t* qos_rl_off;
   const uint8_t* rl_rule;
   const int64_t* rl_value;
@@ -1722,11 +1723,16 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32, ARKS_SSE_MINBLK) scan_sse
 // a work-list entry: text offset | (length - 1) << 32 | body << 40. Entries are handed out 32 at a time (one atomic per flush).
 constexpr int kBpeFlush = 32;
 // Rows whose `row_flags` contain every bit of `wide_mask` count the wide key set (N5 metered rows); row_flags may be null.
+// kDigits: the pre-tokenizer family (bpe_pretokenize). kRows: lane k scans row rows[k] of the first *rows_n (one vocabulary's
+// rows, bpe_split_kernel) instead of row k of n.
+template <uint32_t kDigits, bool kRows>
 __global__ void __launch_bounds__(128) bpe_scan_kernel(const uint8_t* bodies, const uint32_t* body_off, const uint32_t* body_len, uint32_t n,
                                                        BpeTablesDev T, uint8_t* text, unsigned long long* list, uint32_t* list_n,
-                                                       uint32_t list_cap, uint32_t* bpe_out, const uint8_t* row_flags, uint32_t wide_mask) {
-  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
+                                                       uint32_t list_cap, uint32_t* bpe_out, const uint8_t* row_flags, uint32_t wide_mask,
+                                                       const uint32_t* rows, const uint32_t* rows_n) {
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= (kRows ? *rows_n : n)) return;
+  const uint32_t i = kRows ? rows[k] : k;
   const uint32_t off = body_off[i];
   const uint32_t keys = row_flags && (row_flags[i] & wide_mask) == wide_mask ? kBpeKeysWide : kBpeKeysContent;
   unsigned long long buf[kBpeFlush];
@@ -1739,7 +1745,7 @@ __global__ void __launch_bounds__(128) bpe_scan_kernel(const uint8_t* bodies, co
       for (uint32_t k = 0; k < nb; k++) list[at + k] = buf[k];
     nb = 0;
   };
-  const BpeScanOut o = bpe_scan_body(bodies + off, body_len[i], text + off, T, keys, [&](uint32_t s, uint32_t len) {
+  const BpeScanOut o = bpe_scan_body<kDigits>(bodies + off, body_len[i], text + off, T, keys, [&](uint32_t s, uint32_t len) {
     buf[nb++] = (unsigned long long)(off + s) | (unsigned long long)(len - 1) << 32 | (unsigned long long)i << 40;
     if (nb == kBpeFlush) flush();
   });
@@ -1747,8 +1753,10 @@ __global__ void __launch_bounds__(128) bpe_scan_kernel(const uint8_t* bodies, co
   bpe_out[i] = (o.bad || overflow) ? kBpeUncounted : 0u;
 }
 // pass 2: one lane per pre-token (grid-stride over the work list). The hot merges come from shared memory, staged by one
-// bulk copy (TMA) per block; the rest of the merge table is read through L2.
+// bulk copy (TMA) per block; the rest of the merge table is read through L2. kIgnoreMerges: the vocabulary's whole-piece
+// lookup comes first (bpe_piece_tokens).
 constexpr int kBpeMergeThreads = 256;
+template <bool kIgnoreMerges>
 __global__ void __launch_bounds__(kBpeMergeThreads) bpe_merge_kernel(const unsigned long long* list, const uint32_t* list_n, uint32_t list_cap,
                                                                     BpeTablesDev T, const uint8_t* text, uint32_t* bpe_out) {
   __shared__ __align__(128) BpeSlot hot[kBpeHotSlots];
@@ -1766,9 +1774,28 @@ __global__ void __launch_bounds__(kBpeMergeThreads) bpe_merge_kernel(const unsig
     const unsigned long long e = list[k];
     const uint32_t off = (uint32_t)e, len = ((uint32_t)(e >> 32) & 0xffu) + 1u, body = (uint32_t)(e >> 40);
     if (bpe_out[body] == kBpeUncounted) continue;  // written by pass 1, never by this kernel
-    const uint32_t ntok = bpe_piece_tokens(text + off, len, hot, T);
+    const uint32_t ntok = bpe_piece_tokens<kIgnoreMerges>(text + off, len, hot, T);
     atomicAdd(&bpe_out[body], ntok);
   }
+}
+
+// Several vocabularies (arks_bind_model_vocab): every row goes to the list of its qos entry's vocabulary slot (rows without
+// an entry, qos < 0, and rows whose slot is not loaded to slot 0). rows: kBpeMaxVocabs lists of `stride` entries, rows_n:
+// their lengths (zeroed before). One atomic per distinct slot per warp.
+__global__ void __launch_bounds__(128) bpe_split_kernel(const uint8_t* qos_vocab, const int32_t* qos_of, uint32_t n, uint32_t loaded,
+                                                        uint32_t* rows, uint32_t stride, uint32_t* rows_n) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int32_t q = qos_of[i];
+  uint32_t v = q >= 0 ? qos_vocab[q] : 0u;
+  if (v >= kBpeMaxVocabs || !((loaded >> v) & 1u)) v = 0;
+  const uint32_t lane = threadIdx.x & 31u;
+  const unsigned peers = __match_any_sync(__activemask(), v);
+  const uint32_t leader = (uint32_t)__ffs(peers) - 1u;
+  uint32_t at = 0;
+  if (lane == leader) at = atomicAdd(&rows_n[v], (uint32_t)__popc(peers));
+  at = __shfl_sync(peers, at, leader) + (uint32_t)__popc(peers & ((1u << lane) - 1u));
+  rows[(size_t)v * stride + at] = i;
 }
 
 // N5 (arks_set_stream_metering): bills the metered rows of a batch, one lane per row, after the BPE kernels. A row is metered
@@ -1911,9 +1938,15 @@ struct arks_ctx {
   bool qexp_valid = false;
   bool share_quota = false;
   // BPE side output (arks_load_bpe): tables + per-batch scratch
-  bool bpe_on = false;
-  BpeTablesDev bpe{};
-  std::vector<void*> bpe_allocs;
+  bool bpe_on = false;                      // slot 0 (the default vocabulary) is loaded
+  BpeTablesDev bpe[kBpeMaxVocabs]{};        // per vocabulary slot (arks_load_bpe_vocab); slot 0: arks_load_bpe
+  std::vector<void*> bpe_allocs[kBpeMaxVocabs];
+  uint8_t* d_bpe_cls = nullptr;             // the Unicode class table every slot reads (uploaded with slot 0)
+  uint32_t vocab_loaded = 0;                // bit s: slot s holds a vocabulary (bit 0 == bpe_on); written under cfg_mu
+  uint32_t vocab_used = 0;                  // slots other than 0 the current generation's qos entries use (under cfg_mu)
+  bool vocab_multi = false;                 // vocab_used != 0: queue_bpe splits the rows by vocabulary
+  std::unordered_map<std::string, uint32_t> vocab_bind;  // model name -> slot (arks_bind_model_vocab), under cfg_mu
+  uint32_t* d_bpe_rows = nullptr;           // kBpeMaxVocabs row lists of max_batch entries (bpe_split_kernel)
   uint8_t* d_bpe_text = nullptr;            // decoded `content` strings, laid out like the bodies
   unsigned long long* d_bpe_list = nullptr; // work list of pre-tokens
   uint32_t* d_bpe_n = nullptr;
@@ -2164,7 +2197,10 @@ void arks_destroy(arks_ctx* ctx) {
   cudaFree(ctx->d_inter);
   cudaFree(ctx->d_perm);
   cudaFree(ctx->d_slow);
-  for (void* p : ctx->bpe_allocs) cudaFree(p);
+  for (auto& v : ctx->bpe_allocs)
+    for (void* p : v) cudaFree(p);
+  cudaFree(ctx->d_bpe_cls);
+  cudaFree(ctx->d_bpe_rows);
   cudaFree(ctx->d_bpe_text);
   cudaFree(ctx->d_bpe_list);
   cudaFree(ctx->d_bpe_n);
@@ -2238,57 +2274,173 @@ void arks_free_pinned(void* p) {
 }
 
 // ---- BPE side output ------------------------------------------------------------------------------
-int arks_load_bpe(arks_ctx* ctx, const arks_bpe_tables* t) {
-  if (!ctx) return ARKS_E_INVALID_ARG;
-  if (!t && ctx->meter) return fail(ctx, ARKS_E_INVALID_ARG, "stream metering needs the vocabulary: switch it off first");
+static_assert(kBpeMaxVocabs == ARKS_BPE_MAX_VOCABS && kBpeFlagNfc == ARKS_BPE_NFC && kBpeFlagDigits3 == ARKS_BPE_DIGITS3 &&
+                  kBpeFlagIgnoreMerges == ARKS_BPE_IGNORE_MERGES, "include/arks_gateway.h and bpe.cuh disagree");
+// Slot 0 is the default vocabulary (arks_load_bpe); slots 1.. are bound to models by name (arks_bind_model_vocab). Every
+// slot has its own merge / hot / byte-id tables and flags; the Unicode class table is one, uploaded with slot 0.
+int arks_load_bpe_vocab(arks_ctx* ctx, uint32_t slot, const arks_bpe_tables* t, const uint8_t* tok_bytes, const uint32_t* tok_off,
+                        uint32_t n_tok) {
+  if (!ctx || slot >= kBpeMaxVocabs) return ARKS_E_INVALID_ARG;
+  if (!t && slot == 0 && ctx->meter) return fail(ctx, ARKS_E_INVALID_ARG, "stream metering needs the vocabulary: switch it off first");
+  if (!t && slot == 0 && (ctx->vocab_loaded & ~1u)) return fail(ctx, ARKS_E_INVALID_ARG, "other vocabulary slots are loaded: empty them first");
+  if (t && slot != 0 && !ctx->bpe_on) return fail(ctx, ARKS_E_NOT_LOADED, "vocabulary slot %u needs slot 0 (arks_load_bpe) first", slot);
+  if (t && (t->flags & ARKS_BPE_IGNORE_MERGES) && (!tok_off || (n_tok && !tok_bytes)))
+    return fail(ctx, ARKS_E_INVALID_ARG, "ARKS_BPE_IGNORE_MERGES needs the vocabulary's token strings");
+  if (!t) {
+    {
+      // the check and the clearing in one section: a binding that comes after it finds the slot empty (ARKS_E_NOT_LOADED)
+      std::lock_guard<std::mutex> g(ctx->cfg_mu);
+      bool bound = slot != 0 && ((ctx->vocab_used >> slot) & 1u);
+      for (const auto& kv : ctx->vocab_bind) bound |= slot != 0 && kv.second == slot;
+      if (bound)
+        return fail(ctx, ARKS_E_INVALID_ARG, "vocabulary slot %u: a model is bound to it (bind it to slot 0 and publish a generation first)", slot);
+      ctx->vocab_loaded &= ~(1u << slot);
+    }
+    if (slot == 0) ctx->bpe_on = false;
+    CK(cudaSetDevice(ctx->device));
+    CK(cudaStreamSynchronize(ctx->stream));  // batches queued before this call still read the tables
+    for (void* p : ctx->bpe_allocs[slot]) cudaFree(p);
+    ctx->bpe_allocs[slot].clear();
+    return 0;
+  }
+  // A replacement is built completely before the slot's current tables are touched: a refused or failed load leaves the
+  // slot (and the bindings and generations that use it) as they were.
+  if (!t->byte_id || (slot == 0 && !t->cp_class) || (t->n_merges && (!t->left || !t->right || !t->merged)))
+    return fail(ctx, ARKS_E_INVALID_ARG, "incomplete BPE tables");
   CK(cudaSetDevice(ctx->device));
-  CK(cudaStreamSynchronize(ctx->stream));
-  for (void* p : ctx->bpe_allocs) cudaFree(p);
-  ctx->bpe_allocs.clear();
-  ctx->bpe_on = false;
-  if (!t) return 0;
-  if (!t->byte_id || !t->cp_class || (t->n_merges && (!t->left || !t->right || !t->merged))) return fail(ctx, ARKS_E_INVALID_ARG, "incomplete BPE tables");
   std::vector<BpeSlot> table, hot;
   const uint32_t slots = bpe_table_slots(t->n_merges);
   bpe_fill_table(table, slots, t->left, t->right, t->merged, t->n_merges);
   bpe_fill_table(hot, kBpeHotSlots, t->left, t->right, t->merged, t->n_merges < kBpeHotMerges ? t->n_merges : kBpeHotMerges);
-  auto up = [&](const void* src, size_t bytes, const void** out) -> int {
+  std::vector<void*> fresh;
+  auto up = [&](const void* src, size_t bytes, const void** out) -> cudaError_t {
     void* p = nullptr;
-    CK(cudaMalloc(&p, bytes + 64));
-    ctx->bpe_allocs.push_back(p);
-    CK(cudaMemcpy(p, src, bytes, cudaMemcpyHostToDevice));
+    cudaError_t e = cudaMalloc(&p, bytes + 64);
+    if (e != cudaSuccess) return e;
+    fresh.push_back(p);
     *out = p;
-    return 0;
+    return cudaMemcpy(p, src, bytes, cudaMemcpyHostToDevice);
+  };
+  auto drop = [&](cudaError_t e) {
+    for (void* p : fresh) cudaFree(p);
+    return fail(ctx, ARKS_E_CUDA, "arks_load_bpe_vocab: %s (slot %u unchanged)", cudaGetErrorString(e), slot);
   };
   BpeTablesDev d{};
-  int rc;
-  if ((rc = up(t->byte_id, 256 * 4, (const void**)&d.byte_id))) return rc;
-  if ((rc = up(table.data(), table.size() * sizeof(BpeSlot), (const void**)&d.table))) return rc;
-  if ((rc = up(hot.data(), hot.size() * sizeof(BpeSlot), (const void**)&d.hot))) return rc;
-  if ((rc = up(t->cp_class, 0x110000 / 2, (const void**)&d.cp_class))) return rc;
+  cudaError_t e = up(t->byte_id, 256 * 4, (const void**)&d.byte_id);
+  if (e == cudaSuccess) e = up(table.data(), table.size() * sizeof(BpeSlot), (const void**)&d.table);
+  if (e == cudaSuccess) e = up(hot.data(), hot.size() * sizeof(BpeSlot), (const void**)&d.hot);
   d.table_mask = slots - 1;
   d.flags = t->flags;
-  if (!ctx->d_bpe_text) {
-    // a pre-token is rarely shorter than three bytes on average; bodies whose entries do not fit are reported uncounted
-    ctx->bpe_list_cap = (uint32_t)std::min<uint64_t>(ctx->max_bytes / 3 + 1024, 0xfffffff0ull);
-    CK(cudaMalloc(&ctx->d_bpe_text, ctx->max_bytes + 64));
-    CK(cudaMalloc(&ctx->d_bpe_list, (size_t)ctx->bpe_list_cap * 8));
-    CK(cudaMalloc(&ctx->d_bpe_n, 256));
+  if (e == cudaSuccess && (t->flags & ARKS_BPE_IGNORE_MERGES)) {
+    std::vector<BpeWholeSlot> whole;
+    d.whole_mask = bpe_fill_whole(whole, tok_bytes, tok_off, n_tok) - 1;
+    e = up(whole.data(), whole.size() * sizeof(BpeWholeSlot), (const void**)&d.whole);
+    if (e == cudaSuccess) e = up(tok_off, ((size_t)n_tok + 1) * 4, (const void**)&d.whole_off);
+    if (e == cudaSuccess)
+      e = up(n_tok ? (const void*)tok_bytes : (const void*)tok_off, n_tok ? tok_off[n_tok] : 0, (const void**)&d.whole_pool);
   }
-  ctx->bpe = d;
-  ctx->bpe_on = true;
+  // per-context buffers, allocated once and kept
+  if (e == cudaSuccess && !ctx->d_bpe_text) {
+    // a pre-token is rarely shorter than three bytes on average; bodies whose entries do not fit are reported uncounted
+    const uint32_t cap = (uint32_t)std::min<uint64_t>(ctx->max_bytes / 3 + 1024, 0xfffffff0ull);
+    uint8_t* text = nullptr;
+    unsigned long long* list = nullptr;
+    uint32_t* cnt = nullptr;
+    e = cudaMalloc(&text, ctx->max_bytes + 64);
+    if (e == cudaSuccess) e = cudaMalloc(&list, (size_t)cap * 8);
+    if (e == cudaSuccess) e = cudaMalloc(&cnt, 256);
+    if (e == cudaSuccess) {
+      ctx->d_bpe_text = text; ctx->d_bpe_list = list; ctx->d_bpe_n = cnt; ctx->bpe_list_cap = cap;
+    } else {
+      cudaFree(text); cudaFree(list); cudaFree(cnt);
+    }
+  }
+  if (e == cudaSuccess && slot != 0 && !ctx->d_bpe_rows) e = cudaMalloc(&ctx->d_bpe_rows, (size_t)kBpeMaxVocabs * ctx->max_batch * 4 + 64);
+  if (e == cudaSuccess && slot == 0 && !ctx->d_bpe_cls) e = cudaMalloc(&ctx->d_bpe_cls, 0x110000 / 2 + 64);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);  // batches queued before this call still read the old tables
+  if (e == cudaSuccess && slot == 0) e = cudaMemcpy(ctx->d_bpe_cls, t->cp_class, 0x110000 / 2, cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) return drop(e);
+  d.cp_class = ctx->d_bpe_cls;
+  for (void* p : ctx->bpe_allocs[slot]) cudaFree(p);
+  ctx->bpe_allocs[slot] = std::move(fresh);
+  ctx->bpe[slot] = d;
+  if (slot == 0) ctx->bpe_on = true;
+  std::lock_guard<std::mutex> g(ctx->cfg_mu);
+  ctx->vocab_loaded |= 1u << slot;
+  return 0;
+}
+int arks_load_bpe(arks_ctx* ctx, const arks_bpe_tables* t) {
+  if (!ctx) return ARKS_E_INVALID_ARG;
+  if (t && (t->flags & ARKS_BPE_IGNORE_MERGES))
+    return fail(ctx, ARKS_E_INVALID_ARG, "ARKS_BPE_IGNORE_MERGES needs the token strings: use arks_load_bpe_vocab");
+  return arks_load_bpe_vocab(ctx, 0, t, nullptr, nullptr, 0);
+}
+int arks_bind_model_vocab(arks_ctx* ctx, const char* model, uint32_t model_len, uint32_t slot) {
+  if (!ctx || (!model && model_len) || slot >= kBpeMaxVocabs) return ARKS_E_INVALID_ARG;
+  std::lock_guard<std::mutex> g(ctx->cfg_mu);
+  const std::string m(model ? model : "", model_len);
+  if (slot == 0) { ctx->vocab_bind.erase(m); return 0; }
+  if (!((ctx->vocab_loaded >> slot) & 1u)) return fail(ctx, ARKS_E_NOT_LOADED, "vocabulary slot %u is not loaded", slot);
+  ctx->vocab_bind[m] = slot;
   return 0;
 }
 // queue the two BPE kernels for `n` bodies on the compute stream; counts land in bpe_out. Rows whose row_flags (may be null)
 // contain every bit of wide_mask count the wide key set of metered rows
+// row_qos: each row's qos index in the current generation (-1: none), which picks its vocabulary when the generation binds
+// a model to a slot other than 0. Otherwise (one vocabulary) exactly the two kernels over all rows.
 static int queue_bpe(arks_ctx* ctx, const uint8_t* bodies, const uint32_t* body_off, const uint32_t* body_len, uint32_t n, uint32_t* bpe_out,
-                     const uint8_t* row_flags, uint32_t wide_mask) {
-  CK(cudaMemsetAsync(ctx->d_bpe_n, 0, 4, ctx->stream));
-  bpe_scan_kernel<<<(n + 127) / 128, 128, 0, ctx->stream>>>(bodies, body_off, body_len, n, ctx->bpe, ctx->d_bpe_text, ctx->d_bpe_list,
-                                                            ctx->d_bpe_n, ctx->bpe_list_cap, bpe_out, row_flags, wide_mask);
-  bpe_merge_kernel<<<ctx->n_sm * 4, kBpeMergeThreads, 0, ctx->stream>>>(ctx->d_bpe_list, ctx->d_bpe_n, ctx->bpe_list_cap, ctx->bpe,
-                                                                        ctx->d_bpe_text, bpe_out);
-  ctx->launches += 2;
+                     const uint8_t* row_flags, uint32_t wide_mask, const int32_t* row_qos) {
+  if (!ctx->vocab_multi) {
+    // one vocabulary (slot 0), with its own pre-tokenizer family and ignore_merges flag; flags 0 is the Qwen2 pair
+    const BpeTablesDev& T = ctx->bpe[0];
+    CK(cudaMemsetAsync(ctx->d_bpe_n, 0, 4, ctx->stream));
+    if (T.flags & ARKS_BPE_DIGITS3)
+      bpe_scan_kernel<3, false><<<(n + 127) / 128, 128, 0, ctx->stream>>>(bodies, body_off, body_len, n, T, ctx->d_bpe_text, ctx->d_bpe_list,
+                                                                          ctx->d_bpe_n, ctx->bpe_list_cap, bpe_out, row_flags, wide_mask,
+                                                                          nullptr, nullptr);
+    else
+      bpe_scan_kernel<1, false><<<(n + 127) / 128, 128, 0, ctx->stream>>>(bodies, body_off, body_len, n, T, ctx->d_bpe_text, ctx->d_bpe_list,
+                                                                          ctx->d_bpe_n, ctx->bpe_list_cap, bpe_out, row_flags, wide_mask,
+                                                                          nullptr, nullptr);
+    if (T.flags & ARKS_BPE_IGNORE_MERGES)
+      bpe_merge_kernel<true><<<ctx->n_sm * 4, kBpeMergeThreads, 0, ctx->stream>>>(ctx->d_bpe_list, ctx->d_bpe_n, ctx->bpe_list_cap, T,
+                                                                                  ctx->d_bpe_text, bpe_out);
+    else
+      bpe_merge_kernel<false><<<ctx->n_sm * 4, kBpeMergeThreads, 0, ctx->stream>>>(ctx->d_bpe_list, ctx->d_bpe_n, ctx->bpe_list_cap, T,
+                                                                                   ctx->d_bpe_text, bpe_out);
+    ctx->launches += 2;
+    return 0;
+  }
+  // Several vocabularies: the rows are split into one list per slot, then every slot in use runs the two kernels over its
+  // own rows with its own tables. The text buffer and the work list are reused in stream order (a row's decoded text sits
+  // at its body's offset, so the slots never overlap); each slot has its own counters in d_bpe_n: [16 + s] work-list
+  // entries, [32 + s] rows.
+  uint32_t* list_n = ctx->d_bpe_n + 16;
+  uint32_t* rows_n = ctx->d_bpe_n + 32;
+  const uint32_t use = (ctx->vocab_used | 1u) & ctx->vocab_loaded;
+  CK(cudaMemsetAsync(list_n, 0, 32 * 4, ctx->stream));
+  bpe_split_kernel<<<(n + 127) / 128, 128, 0, ctx->stream>>>(ctx->dt.qos_vocab, row_qos, n, use, ctx->d_bpe_rows, ctx->max_batch, rows_n);
+  ctx->launches += 1;
+  for (uint32_t v = 0; v < kBpeMaxVocabs; v++) {
+    if (!((use >> v) & 1u)) continue;
+    const BpeTablesDev& T = ctx->bpe[v];
+    const uint32_t* rows = ctx->d_bpe_rows + (size_t)v * ctx->max_batch;
+    if (T.flags & ARKS_BPE_DIGITS3)
+      bpe_scan_kernel<3, true><<<(n + 127) / 128, 128, 0, ctx->stream>>>(bodies, body_off, body_len, n, T, ctx->d_bpe_text, ctx->d_bpe_list,
+                                                                         list_n + v, ctx->bpe_list_cap, bpe_out, row_flags, wide_mask, rows,
+                                                                         rows_n + v);
+    else
+      bpe_scan_kernel<1, true><<<(n + 127) / 128, 128, 0, ctx->stream>>>(bodies, body_off, body_len, n, T, ctx->d_bpe_text, ctx->d_bpe_list,
+                                                                         list_n + v, ctx->bpe_list_cap, bpe_out, row_flags, wide_mask, rows,
+                                                                         rows_n + v);
+    if (T.flags & ARKS_BPE_IGNORE_MERGES)
+      bpe_merge_kernel<true><<<ctx->n_sm * 4, kBpeMergeThreads, 0, ctx->stream>>>(ctx->d_bpe_list, list_n + v, ctx->bpe_list_cap, T,
+                                                                                  ctx->d_bpe_text, bpe_out);
+    else
+      bpe_merge_kernel<false><<<ctx->n_sm * 4, kBpeMergeThreads, 0, ctx->stream>>>(ctx->d_bpe_list, list_n + v, ctx->bpe_list_cap, T,
+                                                                                   ctx->d_bpe_text, bpe_out);
+    ctx->launches += 2;
+  }
   return 0;
 }
 // queue meter_charge_kernel (N5) on the compute stream, timed on its own when profiling
@@ -2326,6 +2478,7 @@ struct arks_prepared {
   std::vector<int32_t> old_to_new;                          // qos index of the outgoing generation -> this one
   uint32_t base_generation = 0;
   uint32_t n_qos = 0, n_quotas = 0;
+  uint32_t vocab_used = 0;  // vocabulary slots other than 0 its qos entries use (arks_bind_model_vocab at prepare time)
 };
 
 static void free_prepared(arks_ctx* ctx, arks_prepared* p) {
@@ -2416,11 +2569,13 @@ int arks_prepare_tables(arks_ctx* ctx, const arks_tables* t, arks_prepared** out
   std::vector<int32_t> qos_from(t->n_qos + 1, -1), quota_from(t->n_quotas + 1, -1);
   std::vector<int32_t> old_to_new;  // qos index of the outgoing generation -> this one
   uint32_t base_generation;
+  std::unordered_map<std::string, uint32_t> vocab_bind;  // model name -> BPE vocabulary slot, as bound now
   {
     // the only part that looks at the current generation: short, so that a commit on the batch thread never waits for
     // the tens of milliseconds a prepare on the config thread takes
     std::lock_guard<std::mutex> cfg_guard(ctx->cfg_mu);
     base_generation = ctx->generation;
+    vocab_bind = ctx->vocab_bind;
     old_to_new.assign(ctx->loaded ? ctx->ht.n_qos : 0, -1);
   if (ctx->loaded) {
     std::unordered_map<std::string, uint32_t> oq, ou;
@@ -2439,6 +2594,18 @@ int arks_prepare_tables(arks_ctx* ctx, const arks_tables* t, arks_prepared** out
     }
   }
   }
+
+  // the BPE vocabulary of every qos entry, by its model name (the ArksEndpoint name)
+  std::vector<uint8_t> qos_vocab(t->n_qos, 0);
+  uint32_t vocab_used = 0;
+  if (!vocab_bind.empty())
+    for (uint32_t q = 0; q < t->n_qos; q++) {
+      auto it = vocab_bind.find(S(t->qos_model_str[q]));
+      if (it == vocab_bind.end()) continue;
+      qos_vocab[q] = (uint8_t)it->second;
+      vocab_used |= 1u << it->second;
+    }
+  vocab_used &= ~1u;
 
   // Build the new generation completely before touching the old one, on the config stream: a failed allocation or upload
   // leaves the context serving the previous tables and counters, and the data path never waits for any of this.
@@ -2479,6 +2646,7 @@ int arks_prepare_tables(arks_ctx* ctx, const arks_tables* t, arks_prepared** out
   PUT(qmodel_len, qos_model_len);
   PUT(v_qos_quota, qos_quota);
   PUT(qos_ep, qos_ep);
+  PUT(qos_vocab, qos_vocab);
   PUT(v_qos_rl_off, qos_rl_off);
   PUT(v_rl_rule, rl_rule);
   PUT(v_rl_value, rl_value);
@@ -2539,6 +2707,7 @@ int arks_prepare_tables(arks_ctx* ctx, const arks_tables* t, arks_prepared** out
   p->base_generation = base_generation;
   p->n_qos = t->n_qos;
   p->n_quotas = t->n_quotas;
+  p->vocab_used = vocab_used;
   *out = p;
   return 0;
 }
@@ -2552,6 +2721,8 @@ int arks_commit_tables(arks_ctx* ctx, arks_prepared* p) {
   std::lock_guard<std::mutex> cfg_guard(ctx->cfg_mu);
   if (p->base_generation != ctx->generation)
     return fail(ctx, ARKS_E_INVALID_ARG, "prepared against generation %u, the context is at %u: prepare again", p->base_generation, ctx->generation);
+  if (p->vocab_used & ~ctx->vocab_loaded)
+    return fail(ctx, ARKS_E_INVALID_ARG, "prepared with a BPE vocabulary slot that has been emptied since: prepare again");
   if (ctx->loaded) {
     auto carry = [&](long long* dst, const long long* src, const int32_t* map, uint32_t n_new, uint32_t cols, uint32_t ds, uint32_t ss, int cm) {
       if (!dst || !src || !n_new) return;
@@ -2584,6 +2755,8 @@ int arks_commit_tables(arks_ctx* ctx, arks_prepared* p) {
     if (ctx->remap.size() > ARKS_GEN_HISTORY) ctx->remap.pop_front();
   }
   ctx->ht = std::move(p->ht);
+  ctx->vocab_used = p->vocab_used;
+  ctx->vocab_multi = p->vocab_used != 0;
   ctx->generation++;
   ctx->loaded = true;
   delete p;
@@ -3000,7 +3173,7 @@ int arks_run_request_batch(arks_ctx* ctx, int64_t now_unix) {
   if (ctx->prof) CK(cudaEventRecord(ctx->ev[1], ctx->stream));
   if (ctx->bpe_on) {
     if (ctx->prof) CK(cudaEventRecord(ctx->ev_bpe[0], ctx->stream));
-    rc = queue_bpe(ctx, r.bodies, r.body_off, r.body_len, n, r.bpe, ctx->meter ? r.st_flags : nullptr, ARKS_FLAG_METERED);
+    rc = queue_bpe(ctx, r.bodies, r.body_off, r.body_len, n, r.bpe, ctx->meter ? r.st_flags : nullptr, ARKS_FLAG_METERED, r.st_qos);
     if (rc) return rc;
     if (ctx->prof) { CK(cudaEventRecord(ctx->ev_bpe[1], ctx->stream)); ctx->ev_bpe_set = true; }
   }
@@ -3294,7 +3467,7 @@ int arks_run_response_batch(arks_ctx* ctx, int64_t now_unix) {
   if (ctx->bpe_on) {
     if (ctx->prof) CK(cudaEventRecord(ctx->ev_bpe[0], ctx->stream));
     rc = queue_bpe(ctx, sl.rp.bodies, sl.rp.body_off, sl.rp.body_len, n, sl.rp.bpe, sl.resp_metered ? sl.rp.flags : nullptr,
-                   ARKS_RESP_STREAM | ARKS_RESP_METERED);
+                   ARKS_RESP_STREAM | ARKS_RESP_METERED, sl.rp.qos);
     if (rc) return rc;
     if (ctx->prof) { CK(cudaEventRecord(ctx->ev_bpe[1], ctx->stream)); ctx->ev_bpe_set = true; }
   } else {

@@ -20,6 +20,10 @@
 // A body is reported as ARKS_BPE_UNCOUNTED instead of a wrong number when it is outside what this path handles: invalid
 // UTF-8 / escapes, a lone surrogate, a piece longer than kBpeMaxPiece bytes, NFC-unsafe code points when the tokenizer
 // normalises (Qwen2 does), work-list overflow.
+// Two pre-tokenizer families are handled: Qwen2 (one number character per piece) and Llama 3 (runs of up to three, `\p{N}{1,3}`;
+// every other alternative of the two patterns is the same), chosen per vocabulary by kBpeFlagDigits3. A vocabulary with
+// kBpeFlagIgnoreMerges (Llama 3's `"ignore_merges": true`) counts a piece that is itself a vocabulary entry as one token
+// before any merge is tried: the piece's bytes are hashed and compared against the vocabulary's token strings.
 #pragma once
 #include "json_common.cuh"
 
@@ -39,18 +43,29 @@ constexpr uint32_t kBpeHotSlots = 2048;     // shared-memory table: 32 KB, holds
 constexpr uint32_t kBpeHotMerges = ARKS_BPE_HOT_MERGES;
 constexpr uint32_t kBpeUncounted = 0xFFFFFFFFu;
 constexpr uint32_t kBpeFlagNfc = 1u;
+constexpr uint32_t kBpeFlagDigits3 = 2u;        // the pre-tokenizer splits numbers as \p{N}{1,3} (Llama 3) instead of \p{N}
+constexpr uint32_t kBpeFlagIgnoreMerges = 4u;   // a piece that is a vocabulary entry is one token (whole-piece lookup first)
+constexpr uint32_t kBpeMaxVocabs = 8;           // vocabulary slots of a context (slot 0: the default)
 enum : uint32_t { UC_OTHER = 0, UC_LETTER = 1, UC_NUMBER = 2, UC_SPACE = 3, UC_NFC_UNSAFE = 4 };
 
 struct BpeSlot {  // one merge: key = left | right << 32; rank == 0xFFFFFFFF marks an empty slot
   uint32_t left, right, rank, merged;
+};
+struct BpeWholeSlot {  // tok == 0xFFFFFFFF marks an empty slot; fp: the high half of the string's hash
+  uint32_t fp, tok;
 };
 struct BpeTablesDev {
   const uint32_t* byte_id;  // 256
   const BpeSlot* table;     // all merges
   uint32_t table_mask;
   const BpeSlot* hot;       // kBpeHotSlots slots (global image; blocks copy it to shared memory)
-  const uint8_t* cp_class;  // 0x110000 / 2
+  const uint8_t* cp_class;  // 0x110000 / 2 (one table shared by every vocabulary: the classes belong to the pattern)
   uint32_t flags;
+  // kBpeFlagIgnoreMerges only: the vocabulary's token byte strings of 2..kBpeMaxPiece bytes, an open-addressing table over them
+  const BpeWholeSlot* whole = nullptr;
+  uint32_t whole_mask = 0;
+  const uint32_t* whole_off = nullptr;  // token k is whole_pool[whole_off[k], whole_off[k + 1])
+  const uint8_t* whole_pool = nullptr;
 };
 
 // host test build only (tests/host_machine.cpp): counts the table slots a lookup reads, so that the bench can state the
@@ -82,9 +97,34 @@ ARKS_HD bool bpe_lookup(const BpeSlot* hot, const BpeTablesDev& T, uint32_t left
   }
 }
 
+// FNV-1a over a byte string: the whole-piece table's hash (low bits: the slot, high half: the fingerprint)
+ARKS_HD uint64_t bpe_bytes_hash(const uint8_t* p, uint32_t n) {
+  uint64_t h = 0xcbf29ce484222325ull;
+  for (uint32_t i = 0; i < n; i++) h = (h ^ p[i]) * 0x100000001b3ull;
+  return h;
+}
+// the piece is one of the vocabulary's token strings: exact (a fingerprint match is confirmed byte by byte)
+ARKS_HD bool bpe_whole_token(const uint8_t* p, uint32_t n, const BpeTablesDev& T) {
+  const uint64_t h = bpe_bytes_hash(p, n);
+  const uint32_t fp = (uint32_t)(h >> 32);
+  for (uint32_t s = (uint32_t)h & T.whole_mask;; s = (s + 1) & T.whole_mask) {
+    const BpeWholeSlot e = T.whole[s];
+    if (e.tok == 0xFFFFFFFFu) return false;
+    if (e.fp != fp) continue;
+    const uint32_t a = T.whole_off[e.tok];
+    if (T.whole_off[e.tok + 1] - a != n) continue;
+    uint32_t diff = 0;
+    for (uint32_t k = 0; k < n; k++) diff |= (uint32_t)(T.whole_pool[a + k] ^ p[k]);
+    if (diff == 0) return true;
+  }
+}
+
 // tokens of one piece of `n` <= kBpeMaxPiece bytes. Every round looks all adjacent pairs up again instead of keeping their
 // ranks: the same result, a third of the per-lane scratch (pieces are short: a word, a number, a run of punctuation).
+// kIgnoreMerges (vocabularies with kBpeFlagIgnoreMerges): a piece that is a vocabulary entry is one token, merged or not.
+template <bool kIgnoreMerges = false>
 ARKS_HD uint32_t bpe_piece_tokens(const uint8_t* p, uint32_t n, const BpeSlot* hot, const BpeTablesDev& T) {
+  if (kIgnoreMerges && n >= 2 && bpe_whole_token(p, n, T)) return 1;
   uint32_t sym[kBpeMaxPiece];
   for (uint32_t i = 0; i < n; i++) sym[i] = T.byte_id[p[i]];
   while (n > 1) {
@@ -130,7 +170,9 @@ ARKS_HD uint32_t bpe_put_utf8(uint8_t* t, uint32_t w, uint32_t cp) {
 // ---- the Qwen2 split pattern as a scanner over text[s, e) (valid UTF-8); emit(begin, end) per piece, in order ----
 //   (?i:'s|'t|'re|'ve|'m|'ll|'d) | [^\r\n\p{L}\p{N}]?\p{L}+ | \p{N} | ?[^\s\p{L}\p{N}]+[\r\n]* | \s*[\r\n]+ | \s+(?!\S) | \s+
 // Alternatives in order, each greedy with backtracking; checked against `tokenizers` on random Unicode (tests/test_bpe.py).
-template <class E>
+// kDigits: the longest run of number characters alternative 3 takes, 1 (Qwen2: \p{N}) or 3 (Llama 3: \p{N}{1,3}, the only
+// difference between the two patterns; tests/test_model_vocab.py).
+template <uint32_t kDigits = 1, class E>
 ARKS_HD void bpe_pretokenize(const uint8_t* t, uint32_t s, uint32_t e, const uint8_t* cls_tbl, E&& emit) {
   uint32_t i = s;
   auto cls = [&](uint32_t pos, uint32_t* len) { return bpe_class(cls_tbl, bpe_cp_at(t, pos, len)) & 3u; };
@@ -168,8 +210,18 @@ ARKS_HD void bpe_pretokenize(const uint8_t* t, uint32_t s, uint32_t e, const uin
         continue;
       }
     }
-    // 3: one number character
-    if (k0 == UC_NUMBER) { emit(i, i + l0); i += l0; continue; }
+    // 3: one number character (up to kDigits of them)
+    if (k0 == UC_NUMBER) {
+      uint32_t q = i + l0;
+      for (uint32_t d = 1; d < kDigits && q < e; d++) {
+        uint32_t lq;
+        if (cls(q, &lq) != UC_NUMBER) break;
+        q += lq;
+      }
+      emit(i, q);
+      i = q;
+      continue;
+    }
     // 4: an optional space, then characters that are neither white space, letters nor numbers, then newlines
     {
       uint32_t j = i, kj = k0, lj = l0;
@@ -244,8 +296,8 @@ struct BpeScanOut {
   uint32_t bad;     // the body is reported as uncounted
 };
 // text: scratch for the decoded strings of this body (capacity >= len bytes). keys: kBpeKeysContent or kBpeKeysWide.
-// emit(text offset, length) per piece.
-template <class E>
+// emit(text offset, length) per piece. kDigits: the pre-tokenizer family (bpe_pretokenize).
+template <uint32_t kDigits = 1, class E>
 ARKS_HD BpeScanOut bpe_scan_body(const uint8_t* b, uint32_t len, uint8_t* text, const BpeTablesDev& T, uint32_t keys, E&& emit) {
   BpeScanOut o{0, 0};
   uint32_t i = 0, wr = 0;
@@ -308,7 +360,7 @@ ARKS_HD BpeScanOut bpe_scan_body(const uint8_t* b, uint32_t len, uint8_t* text, 
       if (!closed) { o.bad = 1; break; }
       if (count_it) {
         if (unsafe && (T.flags & kBpeFlagNfc)) { o.bad = 1; break; }
-        bpe_pretokenize(text, w0, wr, T.cp_class, [&](uint32_t s, uint32_t e) {
+        bpe_pretokenize<kDigits>(text, w0, wr, T.cp_class, [&](uint32_t s, uint32_t e) {
           if (e - s > kBpeMaxPiece) o.bad = 1;
           else { emit(s, e - s); o.pieces++; }
         });
@@ -355,6 +407,22 @@ inline uint32_t bpe_table_slots(uint32_t n_merges) {
   uint32_t s = 1024;
   while (s < 2 * n_merges + 16) s <<= 1;
   return s;
+}
+// the whole-piece table of a vocabulary with kBpeFlagIgnoreMerges: token k is bytes[off[k], off[k + 1]); only strings of
+// 2..kBpeMaxPiece bytes are entered (shorter or longer pieces never look it up). Returns the slot count (a power of two).
+inline uint32_t bpe_fill_whole(std::vector<BpeWholeSlot>& tab, const uint8_t* bytes, const uint32_t* off, uint32_t n) {
+  uint32_t slots = 1024;
+  while (slots < 2 * n + 16) slots <<= 1;
+  tab.assign(slots, BpeWholeSlot{0, 0xFFFFFFFFu});
+  for (uint32_t k = 0; k < n; k++) {
+    const uint32_t len = off[k + 1] - off[k];
+    if (len < 2 || len > kBpeMaxPiece) continue;
+    const uint64_t h = bpe_bytes_hash(bytes + off[k], len);
+    uint32_t s = (uint32_t)h & (slots - 1);
+    while (tab[s].tok != 0xFFFFFFFFu) s = (s + 1) & (slots - 1);
+    tab[s] = BpeWholeSlot{(uint32_t)(h >> 32), k};
+  }
+  return slots;
 }
 
 }  // namespace arks

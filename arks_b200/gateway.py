@@ -48,6 +48,8 @@ def lib():
         L.arks_last_error.argtypes = [vp]
         L.arks_load_tables.argtypes = [vp, C.POINTER(ArksTables)]
         L.arks_load_bpe.argtypes = [vp, vp]
+        L.arks_load_bpe_vocab.argtypes = [vp, C.c_uint32, vp, abi.u8p, abi.u32p, C.c_uint32]
+        L.arks_bind_model_vocab.argtypes = [vp, C.c_char_p, C.c_uint32, C.c_uint32]
         L.arks_prepare_tables.argtypes = [vp, C.POINTER(ArksTables), C.POINTER(vp)]
         L.arks_commit_tables.argtypes = [vp, vp]
         L.arks_discard_prepared.argtypes = [vp, vp]
@@ -114,7 +116,7 @@ def lib():
 
 EXPORTED = [  # every symbol include/arks_gateway.h declares (checked by tests/test_abi.py)
     "arks_abi_version", "arks_create", "arks_destroy", "arks_last_error", "arks_load_tables", "arks_table_generation", "arks_load_bpe", "arks_set_precharge",
-    "arks_set_stream_metering",
+    "arks_set_stream_metering", "arks_load_bpe_vocab", "arks_bind_model_vocab",
     "arks_prepare_tables", "arks_commit_tables", "arks_discard_prepared", "arks_upsert_token", "arks_delete_token", "arks_upsert_quota",
     "arks_delete_quota", "arks_upsert_endpoint", "arks_delete_endpoint", "arks_config_prepare", "arks_find_quota", "arks_find_qos",
     "arks_update_endpoint_weights", "arks_extract_bearer", "arks_submit_request_batch",
@@ -235,6 +237,23 @@ class Gateway:
             return
         ts = tables.c_struct()
         self._ck(lib().arks_load_bpe(self._h, C.byref(ts)))
+
+    def load_bpe_vocab(self, slot: int, tables):
+        """load a vocabulary (arks_b200.bpe.BpeTables) into slot 0..bpe.MAX_VOCABS-1, or empty the slot with None. Slot 0 is
+        load_bpe's; the others need it and are counted for the models bound to them (bind_model_vocab)"""
+        if tables is None:
+            self._ck(lib().arks_load_bpe_vocab(self._h, slot, None, None, None, 0))
+            return
+        ts = tables.c_struct()
+        tb, to = tables.tok_bytes, tables.tok_off
+        n_tok = 0 if to is None else len(to) - 1
+        self._ck(lib().arks_load_bpe_vocab(self._h, slot, C.byref(ts), abi.ptr(tb, abi.u8p), abi.ptr(to, abi.u32p), n_tok))
+
+    def bind_model_vocab(self, model: str, slot: int):
+        """config thread: count the model's rows with the vocabulary in `slot` (0: remove the binding) from the next
+        generation on (load_tables / commit_tables)"""
+        m = model.encode()
+        self._ck(lib().arks_bind_model_vocab(self._h, m, len(m), slot))
 
     def set_precharge(self, on: bool):
         """N4, opt-in: admitted requests charge their prompt's BPE count to tpm / tpd when their batch commits; responses that

@@ -281,6 +281,11 @@ int32_t arks_find_qos(const arks_ctx* ctx, const char* ns, uint32_t ns_len, cons
  * pre-token longer than 128 bytes, NFC-unsafe text under ARKS_BPE_NFC, work-list overflow). */
 #define ARKS_BPE_UNCOUNTED 0xFFFFFFFFu
 #define ARKS_BPE_NFC 1u  /* flags: the tokenizer normalises to NFC (Qwen2 does): text NFC could change is not counted */
+#define ARKS_BPE_DIGITS3 2u        /* flags: the pre-tokenizer splits numbers as \p{N}{1,3} (Llama 3) instead of \p{N} (Qwen2)  */
+#define ARKS_BPE_IGNORE_MERGES 4u  /* flags: a pre-token that is itself a vocabulary entry is one token, whatever the merges say
+                                    * (the BPE model's "ignore_merges": true, Llama 3); needs the token strings of
+                                    * arks_load_bpe_vocab                                                                  */
+#define ARKS_BPE_MAX_VOCABS 8      /* vocabulary slots per context                                                          */
 typedef struct arks_bpe_tables {
   const uint32_t* byte_id;  /* 256: token id of every single byte (byte-level alphabet)                           */
   uint32_t n_merges;
@@ -291,8 +296,28 @@ typedef struct arks_bpe_tables {
                              * bits 0-1 class (0 other, 1 \p{L}, 2 \p{N}, 3 \s), bit 2 NFC-unsafe; tools/gen_bpe_unicode.py */
   uint32_t flags;
 } arks_bpe_tables;
-/* copies the tables to the device and switches the bpe_count columns on (NULL: off) */
+/* copies the tables to the device and switches the bpe_count columns on (NULL: off). This is vocabulary slot 0, the default
+ * every model is counted with unless it is bound to another slot. Refuses ARKS_BPE_IGNORE_MERGES (no token strings here) and
+ * NULL while another slot is loaded or stream metering is on. */
 int arks_load_bpe(arks_ctx* ctx, const arks_bpe_tables* t);
+/* Per-model vocabularies. A gateway fronts many models, and each should be counted with its own tokenizer (the count feeds
+ * the pre-charge and stream metering). A context holds up to ARKS_BPE_MAX_VOCABS vocabularies; slot 0 is arks_load_bpe's.
+ * arks_load_bpe_vocab loads `t` into `slot` (slot 0: as arks_load_bpe, but ARKS_BPE_IGNORE_MERGES is allowed). With
+ * ARKS_BPE_IGNORE_MERGES, tok_bytes / tok_off are the vocabulary's token strings as bytes (token k is
+ * tok_bytes[tok_off[k], tok_off[k + 1]), n_tok + 1 offsets; only strings of 2..128 bytes matter); otherwise they may be NULL.
+ * All slots share slot 0's Unicode class table: t->cp_class may be NULL for a slot other than 0. A slot other than 0 needs
+ * slot 0 loaded (ARKS_E_NOT_LOADED). t == NULL empties the slot; refused while a model is bound to it, in the bindings or in
+ * the current generation. A load that is refused or fails leaves the slot as it was. Same thread as arks_load_bpe (it waits
+ * for the compute stream). */
+int arks_load_bpe_vocab(arks_ctx* ctx, uint32_t slot, const arks_bpe_tables* t, const uint8_t* tok_bytes, const uint32_t* tok_off,
+                        uint32_t n_tok);
+/* Config thread: count requests and responses of qos entries whose model (the ArksEndpoint name) is `model` with the
+ * vocabulary in `slot`; slot 0 removes the binding. ARKS_E_NOT_LOADED when the slot holds no vocabulary. Bindings are read by
+ * arks_prepare_tables / arks_load_tables / arks_config_prepare and take effect with the NEXT generation; rows without a qos
+ * entry are counted with slot 0. A response row is counted with the binding of the CURRENT generation, the one its qos index
+ * is carried into at staging: a stream whose request was decided under an older generation is counted with today's
+ * vocabulary of its model, and a row whose entry is gone (ARKS_R_QOS_GONE) with slot 0. */
+int arks_bind_model_vocab(arks_ctx* ctx, const char* model, uint32_t model_len, uint32_t slot);
 /* N4 (SURVEY.md section 8f), OPT-IN because it changes admit / deny against the reference, which counts no tokens at request
  * time ("token is not caculated in request", pkg/gateway/check.go:124-126: a tenant over its TPM is only stopped once the
  * upstream has answered). With precharge on and a vocabulary loaded, every ADMITTED request adds its prompt's BPE count to
