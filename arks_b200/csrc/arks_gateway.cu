@@ -1737,12 +1737,19 @@ __global__ void __launch_bounds__(128) bpe_scan_kernel(const uint8_t* bodies, co
   const uint32_t keys = row_flags && (row_flags[i] & wide_mask) == wide_mask ? kBpeKeysWide : kBpeKeysContent;
   unsigned long long buf[kBpeFlush];
   uint32_t nb = 0, overflow = 0;
+  // The counter may run past the capacity (the merge kernel clamps it). A flush that straddles the end still writes the
+  // entries that fit: the merge kernel reads every index below the clamped counter, and a slot this launch left unwritten
+  // would hold an entry of an earlier batch or vocabulary slot, counted against the row it names. The row's own entries
+  // are skipped there (it is reported uncounted).
   auto flush = [&]() {
     if (!nb) return;
     const uint32_t at = atomicAdd(list_n, nb);
-    if (at + nb > list_cap) overflow = 1;  // (the counter may run past the capacity: the merge kernel clamps it)
-    else
+    // (the overflow flag is set apart from the two loops: with it inside the second branch the digits3 instantiations spill)
+    if (at + nb > list_cap) overflow = 1;
+    if (at + nb <= list_cap)
       for (uint32_t k = 0; k < nb; k++) list[at + k] = buf[k];
+    else
+      for (uint32_t k = 0; at + k < list_cap; k++) list[at + k] = buf[k];  // at + nb > list_cap: k stays below nb
     nb = 0;
   };
   const BpeScanOut o = bpe_scan_body<kDigits>(bodies + off, body_len[i], text + off, T, keys, [&](uint32_t s, uint32_t len) {
@@ -2341,7 +2348,10 @@ int arks_load_bpe_vocab(arks_ctx* ctx, uint32_t slot, const arks_bpe_tables* t, 
   }
   // per-context buffers, allocated once and kept
   if (e == cudaSuccess && !ctx->d_bpe_text) {
-    // a pre-token is rarely shorter than three bytes on average; bodies whose entries do not fit are reported uncounted
+    // The work list holds max_bytes / 3 + 1024 entries (one per pre-token) per batch and vocabulary slot: a pre-token is
+    // rarely shorter than three bytes on average, but digits and "1 2 3" style text make about one per byte. A row whose
+    // entries do not all fit is reported ARKS_BPE_UNCOUNTED (which rows: the order lanes reach the list). Such a row
+    // gets no N4 pre-charge and, when metered (N5), is billed its body length.
     const uint32_t cap = (uint32_t)std::min<uint64_t>(ctx->max_bytes / 3 + 1024, 0xfffffff0ull);
     uint8_t* text = nullptr;
     unsigned long long* list = nullptr;
