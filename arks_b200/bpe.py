@@ -234,6 +234,14 @@ def standin_tokenizer(vocab_size: int = 151_643, seed: int = 0xB9E, cache_dir: s
     tok.train_from_iterator(_corpus(60_000 if vocab_size < 50_000 else 300_000, seed), trainer)
     text = tok.to_str()
     if path:
-        os.makedirs(cache_dir, exist_ok=True)
-        open(path, "w").write(text)
+        # the cache only saves the training time: a directory that cannot be written (a read-only checkout) is not an error
+        tmp = f"{path}.{os.getpid()}.tmp"
+        try:
+            os.makedirs(cache_dir, exist_ok=True)
+            with open(tmp, "w") as f:
+                f.write(text)
+            os.replace(tmp, path)  # readers never see a half-written file
+        except OSError:
+            if os.path.exists(tmp):
+                os.unlink(tmp)
     return tok, text

@@ -1324,13 +1324,13 @@ __device__ __forceinline__ void warp_agg_add(long long* addr, long long v, bool 
   if (!active) return;
   unsigned peers = __match_any_sync(mask, (unsigned long long)addr);
   int leader = __ffs(peers) - 1;
-  long long sum = 0;
+  unsigned long long sum = 0;  // counters wrap like the reference's int64 INCRBY: add modulo 2^64
   // reduce over the peer set (peers differ per lane group; iterate set bits)
   for (unsigned p = peers; p; p &= p - 1) {
     int src = __ffs(p) - 1;
-    sum += __shfl_sync(peers, v, src);
+    sum += (unsigned long long)__shfl_sync(peers, v, src);
   }
-  if ((int)(threadIdx.x & 31) == leader) atomicAdd(reinterpret_cast<unsigned long long*>(addr), (unsigned long long)sum);
+  if ((int)(threadIdx.x & 31) == leader) atomicAdd(reinterpret_cast<unsigned long long*>(addr), sum);
 }
 
 // What A11 needs to know about a qos entry: how many of its rate-limit rules are tpm / tpd and how many items of each
@@ -1388,17 +1388,19 @@ __device__ __forceinline__ void account_usage(const DevTables& T, const RespDev&
   }
   // doTokenRateLimit: += total on every token-type entry (check.go:47-59). Warp-aggregated per address.
   const int32_t qt = counted ? acct.qt : ARKS_QUOTA_NONE;
-  const long long pre = B.precharged && live ? (long long)B.precharged[i] : 0;  // N4: the request phase's estimate is reconciled
+  // N4: the request phase's estimate is reconciled. Modulo 2^64 like every counter: u2 may be INT64_MIN
+  const unsigned long long pre = B.precharged && live ? B.precharged[i] : 0u;
 #pragma unroll
   for (int r = 0; r < 2; r++)
-    warp_agg_add(T.rate + (size_t)(2 + r) * T.n_qos + qos, (u2 - pre) * (long long)acct.nt[r], counted && acct.nt[r]);
+    warp_agg_add(T.rate + (size_t)(2 + r) * T.n_qos + qos, (long long)(((unsigned long long)u2 - pre) * (unsigned long long)acct.nt[r]),
+                 counted && acct.nt[r]);
   // doTokenQuotaLimit: QosToQuotaRequests + IncrUsage (check.go:62-72, qosconfig/types.go:45-72)
   long long add[3] = {0, 0, 0};
   if (counted && qt == ARKS_QUOTA_MISSING) reason = ARKS_R_QUOTA_CONFIG_RESP;
   if (counted && qt >= 0) {
-    add[0] = u0 * (long long)acct.nq[0];
-    add[1] = u1 * (long long)acct.nq[1];
-    add[2] = u2 * (long long)acct.nq[2];
+    add[0] = (long long)((unsigned long long)u0 * (unsigned long long)acct.nq[0]);
+    add[1] = (long long)((unsigned long long)u1 * (unsigned long long)acct.nq[1]);
+    add[2] = (long long)((unsigned long long)u2 * (unsigned long long)acct.nq[2]);
   }
 #pragma unroll
   for (int ty = 0; ty < 3; ty++)

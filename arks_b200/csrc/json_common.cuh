@@ -216,22 +216,91 @@ static ARKS_OUTLINE uint64_t struct_key_hash_slow(const uint8_t* p, uint32_t n) 
   decode_span(p + i, n - i, [&](uint8_t b) { h = fhash_step(h, b); });
   return h;
 }
-// gjson Result.Int for a Number token from its captured pieces
-static ARKS_OUTLINE int64_t captured_number_value(uint64_t nacc, uint32_t nneg, uint32_t nplain, uint32_t novf, int32_t nfrac,
-                                                   int32_t nexp, uint32_t nexpneg) {
-  if (nplain) return nneg ? (int64_t)(0 - nacc) : (int64_t)nacc;  // safeInt / parseInt agree with a wrapping parse
-  // mantissa * 10^(exp - frac) truncated toward zero; exact for the documented domain (<= 18 digits)
-  int64_t e10 = (int64_t)(nexpneg ? -nexp : nexp) - (int64_t)nfrac;
-  uint64_t m = nacc;
-  bool ovf = novf;
-  if (m == 0) return 0;
-  while (e10 < 0 && m) { m /= 10; e10++; }
-  while (e10 > 0 && !ovf) {
-    if (m > 0xFFFFFFFFFFFFFFFFull / 10) ovf = true; else m *= 10;
-    e10--;
+// gjson Result.Int of a Number token with a fraction or an exponent, re-read from its raw bytes p[0, n) (the validated
+// number, possibly followed by bytes that cannot belong to it): int64(strconv.ParseFloat(raw, 64)) as Go computes it on
+// amd64. That is the exact decimal value rounded to the nearest double (ties to even) and truncated toward zero, or
+// INT64_MIN when the double is outside [-2^63, 2^63). Computed exactly with integer arithmetic for numbers of any
+// length; only the exponent saturates the way ParseFloat's does (it stops growing at 10000), which can change a result
+// for numbers of thousands of bytes and more only.
+ARKS_HD uint32_t clz64(uint64_t x) {
+#if defined(__CUDA_ARCH__)
+  return (uint32_t)__clzll((long long)x);
+#else
+  return (uint32_t)__builtin_clzll(x);
+#endif
+}
+static ARKS_OUTLINE int64_t float_number_value(const uint8_t* p, uint32_t n) {
+  uint32_t i = 0;
+  const bool neg = n > 0 && p[0] == '-';
+  if (neg) i++;
+  const uint32_t i0 = i;  // integer digits [i0, i1), fraction digits [f0, f0 + (m - ni))
+  while (i < n && is_digit(p[i])) i++;
+  const uint32_t i1 = i, ni = i1 - i0;
+  uint32_t f0 = i;
+  if (i < n && p[i] == '.') {
+    f0 = ++i;
+    while (i < n && is_digit(p[i])) i++;
   }
-  if (ovf || m > 0x7FFFFFFFFFFFFFFFull) return INT64_MIN;
-  return nneg ? -(int64_t)m : (int64_t)m;
+  const int64_t m = (int64_t)ni + (int64_t)(i - f0);  // mantissa digits
+  int64_t e = 0;
+  if (i < n && (p[i] | 0x20) == 'e') {
+    i++;
+    const bool eneg = i < n && p[i] == '-';
+    if (i < n && (p[i] == '-' || p[i] == '+')) i++;
+    for (; i < n && is_digit(p[i]); i++)
+      if (e < 10000) e = e * 10 + (p[i] - '0');
+    if (eneg) e = -e;
+  }
+  // k-th mantissa digit (0 outside the mantissa)
+  auto dig = [&](int64_t k) -> uint32_t {
+    if (k < 0 || k >= m) return 0;
+    return (uint32_t)(k < ni ? p[i0 + k] : p[f0 + (k - ni)]) - '0';
+  };
+  int64_t z = 0, l = m - 1;  // first and last nonzero mantissa digit
+  while (z < m && dig(z) == 0) z++;
+  if (z == m) return 0;
+  while (dig(l) == 0) l--;
+  // value = 0.d_z d_z+1 ... d_l * 10^P: the integer part is mantissa digits [z, z + P), the fraction the ones after
+  const int64_t P = (int64_t)ni + e - z;
+  if (P > 19) return INT64_MIN;  // >= 10^19 > 2^63
+  uint64_t N = 0;
+  for (int64_t k = z; k < z + P; k++) N = N * 10 + dig(k);
+  if (N >> 63) return INT64_MIN;
+  const int64_t f = z + P;    // index of the first fraction digit
+  const bool frac = l >= f;   // the fraction is not zero
+  uint64_t r;
+  if (N >> 53) {
+    // doubles here are the multiples of 2^s: round the low s bits plus the fraction to nearest, ties to even
+    const uint32_t s = 63 - clz64(N) - 52;
+    const uint64_t low = N & ((1ull << s) - 1), half = 1ull << (s - 1), q = N >> s;
+    const bool up = low > half || (low == half && (frac || (q & 1)));
+    r = (q + up) << s;
+    if (r >> 63) return INT64_MIN;
+  } else {
+    // the result is N or N + 1. N + 1 = n with 2^k < n <= 2^(k+1) is a double, and so is its predecessor n - 2^(k-52):
+    // the value rounds to n iff its fraction is >= 1 - 2^-j with j = 53 - k, on a tie iff n's mantissa is even, which
+    // holds for every n up to 2^52 and for even n above
+    const uint32_t bl = N ? 64 - clz64(N) : 0, j = 54 - bl;  // k = bl - 1
+    const uint64_t den = 1ull << j;
+    uint64_t rem = den - 1;  // the digits of (2^j - 1) / 2^j by long division: exactly j of them
+    int cmp = 0;
+    int64_t k = f;
+    for (; rem != 0 && cmp == 0; k++) {
+      rem *= 10;
+      const uint32_t t = (uint32_t)(rem >> j), d = dig(k);
+      rem &= den - 1;
+      cmp = d > t ? 1 : d < t ? -1 : 0;
+    }
+    if (cmp == 0) cmp = l >= k ? 1 : 0;  // digits beyond the threshold's last one
+    r = N + (cmp > 0 || (cmp == 0 && (j >= 2 || (N & 1))));
+  }
+  return neg ? (int64_t)(0 - r) : (int64_t)r;
+}
+// gjson Result.Int for a Number token: a plain integer from its streamed capture (safeInt and parseInt both agree with a
+// wrapping parse), anything else from its raw bytes
+static ARKS_OUTLINE int64_t captured_number_value(uint64_t nacc, uint32_t nneg, uint32_t nplain, const uint8_t* p, uint32_t n) {
+  if (nplain) return nneg ? (int64_t)(0 - nacc) : (int64_t)nacc;
+  return float_number_value(p, n);
 }
 
 // ---------------------------------------------------------------------------------------------

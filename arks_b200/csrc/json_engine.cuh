@@ -37,9 +37,8 @@ enum : uint32_t { KK_NONE = 0, KK_STRUCT = 1, KK_EXACT = 2 };   // keys that are
 struct JsonCold {
   int64_t usage[3];  // prompt, completion, total
   int64_t cand[3];   // candidates of the usage object being read (committed when it closes)
-  uint64_t nacc;     // number / string-number capture (gjson Result.Int)
-  int32_t nfrac, nexp;
-  uint32_t nneg, nplain, novf, ncphase, nexpneg, sval_ok, sval_any;
+  uint64_t nacc;     // number / string-number capture (gjson Result.Int); a number's start is in JsonT::sstart
+  uint32_t nneg, nplain, sval_ok, sval_any;
   uint32_t cand_set, cand_nonnull;
   uint32_t m_start, m_rawlen, m_esc;  // raw span of the model string
   uint32_t stream3, so_present, iu3;  // tri-states: 0 nil, 1 false, 2 true
@@ -80,8 +79,8 @@ struct JsonT {
     hb = k;
     c->usage[0] = c->usage[1] = c->usage[2] = 0;
     c->cand[0] = c->cand[1] = c->cand[2] = 0;
-    c->nacc = 0; c->nfrac = 0; c->nexp = 0;
-    c->nneg = 0; c->nplain = 1; c->novf = 0; c->ncphase = 0; c->nexpneg = 0; c->sval_ok = 0; c->sval_any = 0;
+    c->nacc = 0;
+    c->nneg = 0; c->nplain = 1; c->sval_ok = 0; c->sval_any = 0;
     c->cand_set = 0; c->cand_nonnull = 0;
     c->m_start = 0; c->m_rawlen = 0; c->m_esc = 0; c->stream3 = 0; c->so_present = 0; c->iu3 = 0;
     c->has_error_key = 0; c->n_choices = 0;
@@ -159,7 +158,8 @@ struct JsonT {
         q->nacc = 0; q->nneg = 0; q->sval_ok = 1; q->sval_any = 0;
       } else if (c == '-' || is_digit(c)) {
         set_ncap(2);  // armed: this very byte is the number's first byte; it is captured when it is re-dispatched
-        q->nneg = 0; q->nacc = 0; q->nplain = 1; q->novf = 0; q->nfrac = 0; q->nexp = 0; q->nexpneg = 0; q->ncphase = 0;
+        sstart = pos;  // no string is open while a number is captured
+        q->nneg = 0; q->nacc = 0; q->nplain = 1;
       }
       return false;
     }
@@ -244,7 +244,7 @@ struct JsonT {
     pop();
     ss = depth == 0 ? TS_FINISH : TS_AFTER_A + top_ctx();
   }
-  // a byte of a captured number
+  // a byte of a captured number: a plain integer is parsed on the fly (wrapping), anything else is re-read at its end
   ARKS_HD void capture_number_byte(uint8_t c) {
     JsonCold* q = cold;
     if (ncap() == 2) {  // the number's first byte
@@ -252,25 +252,14 @@ struct JsonT {
       if (c == '-') q->nneg = 1; else q->nacc = (uint64_t)(c - '0');
       return;
     }
-    if (is_digit(c)) {
-      if (q->ncphase == 2) {
-        if (q->nexp < 100000) q->nexp = q->nexp * 10 + (c - '0');
-      } else {
-        if (q->nacc > (0xFFFFFFFFFFFFFFFFull - 9) / 10) q->novf = 1;
-        q->nacc = q->nacc * 10 + (uint64_t)(c - '0');
-        if (q->ncphase == 1) q->nfrac++;
-      }
-    } else {
-      q->nplain = 0;
-      if (c == '.') q->ncphase = 1;
-      else if (c == 'e' || c == 'E') q->ncphase = 2;
-      else if (c == '-' && q->ncphase == 2) q->nexpneg = 1;
-    }
+    if (is_digit(c)) q->nacc = q->nacc * 10 + (uint64_t)(c - '0');
+    else q->nplain = 0;
   }
-  ARKS_HD void finish_number_capture() {
+  // `pos`: the byte after the number (a CR held back by the SSE line layer can make it one more)
+  ARKS_HD void finish_number_capture(uint32_t pos) {
     JsonCold* q = cold;
     set_ncap(0);
-    q->cand[ufield()] = captured_number_value(q->nacc, q->nneg, q->nplain, q->novf, q->nfrac, q->nexp, q->nexpneg);
+    q->cand[ufield()] = captured_number_value(q->nacc, q->nneg, q->nplain, base + sstart, pos - sstart);
   }
   // side work of an ordinary (non-event) transition while something is being captured
   ARKS_HD void side_work(uint32_t ps, uint8_t c, uint32_t pos) {
@@ -309,7 +298,7 @@ struct JsonT {
         if (((vm() != VM_SKIP) | (ps == TS_VAL_T)) && special_value_begin(c, pos, ps)) return;
         ss = ps == TS_VAL_S ? TS_VALG_S : ps == TS_VAL_X ? TS_VALG_X : TS_VALG_T;
       } else if (t == EV_NUM_DONE) {
-        if (ncap()) finish_number_capture();
+        if (ncap()) finish_number_capture(pos);
         ss = TS_AFTER_X;
       } else {  // EV_CHOICE_ELEM
         cold->n_choices = 1;

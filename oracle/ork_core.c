@@ -558,7 +558,7 @@ static void handle_response_inner(ork* o, const arks_response_batch* b, arks_res
     for (uint32_t j = o->qos_rl_off[q]; j < o->qos_rl_off[q + 1]; j++) {
       int rule = o->rl_rule[j];
       if (!RULE_IS_REQUEST[rule]) /* N4: minus what the request phase charged for this stream, if the host says so */
-        rate_incr(o, (uint32_t)q, rule, ork_window_start(b->now_unix, rule), usage[2] - (b->precharged ? (int64_t)b->precharged[i] : 0));
+        rate_incr(o, (uint32_t)q, rule, ork_window_start(b->now_unix, rule), (int64_t)((uint64_t)usage[2] - (b->precharged ? (uint64_t)b->precharged[i] : 0)));
     }
     /* doTokenQuotaLimit: QosToQuotaRequests(conf, countMap) -> IncrUsage   check.go:62-72 */
     int32_t qt = o->qos_quota[q];

@@ -18,8 +18,10 @@
  *   D1  numbers in *skipped* positions: jsoniter's trySkipNumber is restated exactly; when it defers to
  *       ReadFloat64/ReadBigFloat we validate the RFC 8259 number grammar instead of Go's ParseFloat
  *       (differs only for malformed numbers such as "+1", "1.", or magnitudes beyond float range).
- *   D2  usage counters written with a fraction/exponent are converted with strtod + truncation
- *       (gjson Result.Int); out-of-int64-range conversions yield INT64_MIN (amd64 behaviour).
+ *   D2  usage counters written with a fraction/exponent are converted with strtod over the whole number +
+ *       truncation (gjson Result.Int); out-of-int64-range conversions yield INT64_MIN (amd64 behaviour).
+ *       strtod does not stop growing the exponent at 10000 as ParseFloat does: only numbers thousands of
+ *       bytes long can tell the two apart.
  */
 #include <math.h>
 #include <stdlib.h>
@@ -708,14 +710,17 @@ static int64_t gj_int(const uint8_t* b, size_t i, size_t e) {
       gj_parse_int(b + i, e - i, &out);
       return out;
     }
-    char tmp[512];
-    size_t L = e - i < sizeof tmp - 1 ? e - i : sizeof tmp - 1;
-    memcpy(tmp, b + i, L);
-    tmp[L] = 0;
+    /* ParseFloat reads the whole number: strtod is correctly rounded too, given all of it */
+    char buf[64];
+    char* tmp = e - i < sizeof buf ? buf : (char*)malloc(e - i + 1);
+    if (!tmp) abort();
+    memcpy(tmp, b + i, e - i);
+    tmp[e - i] = 0;
     double f = strtod(tmp, NULL);
+    if (tmp != buf) free(tmp);
     if (f >= -9007199254740991.0 && f <= 9007199254740991.0) return (int64_t)f;
     if (f >= -9223372036854775808.0 && f < 9223372036854775808.0) return (int64_t)f;
-    return INT64_MIN; /* D2 */
+    return INT64_MIN; /* int64(f) on amd64, +-Inf included */
   }
   return 0; /* False, Null (never reached: nulls are skipped by apijson), JSON */
 }

@@ -12,8 +12,6 @@ from jsonfuzz import Gen
 from arks_b200 import abi, traffic
 from arks_b200.abi import RequestBatch, ResponseBatch
 from arks_b200.gateway import Gateway
-import re
-D2 = re.compile(rb"[0-9.]{17,}|[eE][+-]?[0-9]{2,}")  # D2 of DESIGN.md §4: very long / large-exponent numbers are outside the pinned domain
 
 rounds = int(sys.argv[1]) if len(sys.argv) > 1 else 20
 seed = int(sys.argv[2]) if len(sys.argv) > 2 else 1
@@ -35,9 +33,7 @@ for r in range(rounds):
         bodies = [bytes(req.bodies[req.body_off[i]:req.body_off[i] + req.body_len[i]]) for i in range(req.n)]
         toks = [bytes(req.tokens[req.token_off[i]:req.token_off[i + 1]]) for i in range(req.n)]
         for i in rng.integers(0, req.n, req.n // 10):
-            b = gen.request()
-            if not D2.search(b):
-                bodies[int(i)] = b
+            bodies[int(i)] = gen.request()
         req = RequestBatch.from_lists(bodies, toks, now, pick_rand=req.pick_rand)
     a, b = g.handle_request_body(req), o.request_batch(req)
     same(a, b, f"round {r} request")
@@ -48,9 +44,7 @@ for r in range(rounds):
         fl = resp.flags.copy()
         for i in rng.integers(0, resp.n, resp.n // 10):
             i = int(i)
-            d = gen.sse_chunk() if fl[i] & abi.RESP_STREAM else gen.response()
-            if not D2.search(d):
-                bodies[i] = d
+            bodies[i] = gen.sse_chunk() if fl[i] & abi.RESP_STREAM else gen.response()
         fl = np.where(fl & abi.RESP_STREAM, fl | rng.choice([0, 2, 4, 6], resp.n).astype(np.uint8), fl)
         kinds = [None] if rng.random() < 0.4 else [0, 1]     # mixed batch, or split into JSON-only / SSE-only batches
         for kind in kinds:

@@ -15,6 +15,7 @@ Every function returns None when a document is OUTSIDE the subset on which these
 libraries are known to agree (invalid UTF-8, lone surrogates, non-integer counters, id:/retry: lines, lone CR, ...);
 the pin tests skip those and count how many documents took part. TEST INFRASTRUCTURE."""
 import json
+import re
 
 I64 = (-(1 << 63), (1 << 63) - 1)
 
@@ -145,6 +146,39 @@ def _usage_into(v, usage):
         else:
             return False  # floats, strings, containers, out-of-range integers: gjson specifics, outside the subset
     return True
+
+
+INT64_MIN = I64[0]
+_PLAIN_INT = re.compile(rb"-?[0-9]+")
+
+
+def _wrap64(v: int) -> int:
+    return (v + (1 << 63)) % (1 << 64) - (1 << 63)
+
+
+def _gjson_parse_int(s: bytes) -> int:
+    """gjson parseInt: `-?[0-9]+` read into an int64 that wraps; anything else is 0"""
+    if not _PLAIN_INT.fullmatch(s):
+        return 0
+    return _wrap64(int(s))
+
+
+def gjson_int(raw: bytes) -> int:
+    """gjson Result.Int of a usage counter's raw JSON token (a number, or a string without escapes), stated with Python's
+    int and float only. A plain integer is the wrapping int64 parse. Any other number is safeInt(ParseFloat(raw)) when
+    |f| <= 2^53-1, else int64(f), which on amd64 is INT64_MIN outside [-2^63, 2^63) and for +-Inf. float() rounds
+    correctly like ParseFloat; ParseFloat's exponent stops growing at 10000, which cannot matter for numbers of up to
+    4 KiB of text, the domain this rule is stated for. A string is parseInt of its raw content."""
+    if raw[:1] == b'"':
+        return _gjson_parse_int(raw[1:-1])
+    if _PLAIN_INT.fullmatch(raw):
+        return _gjson_parse_int(raw)
+    f = float(raw)
+    if abs(f) <= (1 << 53) - 1:
+        return int(f)
+    if -(1 << 63) <= f < (1 << 63):
+        return int(f)
+    return INT64_MIN
 
 
 def response_fields(body: bytes):

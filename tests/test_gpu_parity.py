@@ -1,8 +1,6 @@
 """GPU parity: the CUDA path, called through the C ABI, against the oracle on the same seeded inputs.
 Bit-exact on every output array (reason, detail, flags, qos, token, pick, currentUsage, limitMax, usage ints,
 counted) and on the counter snapshots (rate windows, quota usage) after every batch."""
-import re
-
 import numpy as np
 import pytest
 
@@ -14,7 +12,6 @@ from jsonfuzz import Gen
 
 pytestmark = pytest.mark.gpu
 NOW = 1_700_000_000
-D2 = re.compile(rb"[0-9.]{17,}|[eE][+-]?[0-9]{2,}")
 
 
 def pair(gwmod, tables, max_batch=4096, max_bytes=16 << 20):
@@ -141,8 +138,6 @@ def test_fuzzed_response_bodies_and_sse(gwmod, seed):
             b, f = gen.response(), abi.RESP_END_OF_STREAM
         else:
             b, f = gen.sse_chunk(), abi.RESP_STREAM
-        if D2.search(b):
-            continue
         bodies.append(b)
         flags.append(f if gen.r.random() < 0.97 else 0)
     resp = ResponseBatch.from_lists(bodies, [i % 8 for i in range(4000)], flags, NOW)
@@ -191,8 +186,6 @@ def test_all_sse_batches_event_parallel_kernel(gwmod, seed):
             b = b"".join(b"data: {}\n\n" if r.random() < 0.9 else b"data: " + usage_ev % (1, 2, 3) + b"\n\n" for _ in range(n))
         else:
             b = b"data: " + delta_ev % (b"x" * r.randint(100, 3000)) + b"\n\n" + b"data: " + usage_ev % (7, 8, 15) + b"\n\n"
-        if D2.search(b):
-            continue
         bodies.append(b)
     for lo in range(0, 6000, 3000):
         part = bodies[lo:lo + 3000]
@@ -304,10 +297,8 @@ def test_two_stage_scan_fuzzed_and_plain_documents(gwmod):
     # complete response bodies (a homogeneous JSON batch takes the two-stage path too)
     rb, flags = [], []
     while len(rb) < 5000:
-        b = gen.response()
-        if not D2.search(b):
-            rb.append(b)
-            flags.append(abi.RESP_END_OF_STREAM if gen.r.random() < 0.97 else 0)
+        rb.append(gen.response())
+        flags.append(abi.RESP_END_OF_STREAM if gen.r.random() < 0.97 else 0)
     for _ in range(4000):
         rb.append(traffic.chat_response_body_varied(rng, int(rng.integers(50, 401)), int(rng.integers(1, 513)), 600))
         flags.append(abi.RESP_END_OF_STREAM)
@@ -353,10 +344,8 @@ def test_latency_path_warp_per_body_fuzzed(gwmod, seed):
         same(a, o.request_batch(req), f"warp path requests n={n}")
         rb, flags = [], []
         while len(rb) < n:
-            b = gen.response() if rng.random() < 0.5 else traffic.chat_response_body_varied(rng, 10, 20, 600)
-            if not D2.search(b):
-                rb.append(b)
-                flags.append(abi.RESP_END_OF_STREAM if rng.random() < 0.95 else 0)
+            rb.append(gen.response() if rng.random() < 0.5 else traffic.chat_response_body_varied(rng, 10, 20, 600))
+            flags.append(abi.RESP_END_OF_STREAM if rng.random() < 0.95 else 0)
         resp = ResponseBatch.from_lists(rb, [int(i) % 8 if i % 13 else -1 for i in range(n)], flags, now + 1)
         c = g.handle_response_body(resp)
         same(c, o.response_batch(resp), f"warp path responses n={n}")

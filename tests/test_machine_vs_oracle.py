@@ -1,24 +1,13 @@
 """Differential fuzz on CPU: the device byte state machines (arks_b200/csrc/json_engine.cuh, compiled for the host
 by tests/host_machine.cpp) against the oracle's function-by-function restatement of jsoniter / ssestream / gjson
-(oracle/ork_json.c). Any disagreement on (error?, model bytes, stream flags, usage ints) fails.
-
-Documents containing a usage-shaped number with a fraction/exponent and more than 15 significant digits are outside
-the documented exact domain (divergence D2, DESIGN.md §4) and are skipped."""
+(oracle/ork_json.c). Any disagreement on (error?, model bytes, stream flags, usage ints) fails."""
 import random
-import re
 
 import pytest
 
 import hostmachine as hm
 import orklib
 from jsonfuzz import Gen
-
-D2 = re.compile(rb"[0-9.]{17,}|[eE][+-]?[0-9]{2,}")
-
-
-def d2(b):
-    return bool(D2.search(b))
-
 
 @pytest.mark.parametrize("seed", [11, 12])
 def test_request_body_machine(seed):
@@ -34,8 +23,6 @@ def test_response_body_machine(seed):
     g = Gen(seed)
     for _ in range(30000):
         b = g.response()
-        if d2(b):
-            continue
         a, c = orklib.parse_response_body(b), hm.parse_response_body(b)
         assert a[0] == c[0], (b, a, c)
         if a[0] == 0:
@@ -47,8 +34,6 @@ def test_sse_chunk_machine(seed):
     g = Gen(seed)
     for _ in range(30000):
         b = g.sse_chunk()
-        if d2(b):
-            continue
         a, c = orklib.parse_sse_chunk(b), hm.parse_sse_chunk(b)
         assert a[0] == c[0] and (a[0] == 1 or a == c), (b, a, c)
 
@@ -65,8 +50,6 @@ def test_sse_chunk_split_path(seed):
             b = b.replace(b"\r\n", b"\n").replace(b"data:  ", b"data: ")
         if it % 7 == 0:
             b = b": ping\n\n".join([b] * 1) + b""
-        if d2(b):
-            continue
         a = orklib.parse_sse_chunk(b)
         rc, usage, fell_back = hm.parse_sse_chunk_split(b)
         n_irr += fell_back
@@ -115,18 +98,15 @@ def test_other_schedules_same_results(mode):
         g = Gen(41 + mode)
         for _ in range(8000):
             b = g.request()
-            if not d2(b):
-                a, c = orklib.parse_request_body(b), hm.parse_request_body(b)
-                assert a[0] == c[0] and (a[0] == 1 or a == c), (b, a, c)
+            a, c = orklib.parse_request_body(b), hm.parse_request_body(b)
+            assert a[0] == c[0] and (a[0] == 1 or a == c), (b, a, c)
             b = g.response()
-            if not d2(b):
-                a, c = orklib.parse_response_body(b), hm.parse_response_body(b)
-                assert a[0] == c[0] and (a[0] == 1 or (a[1] > 0, a[2]) == (c[1] > 0, c[2])), (b, a, c)
+            a, c = orklib.parse_response_body(b), hm.parse_response_body(b)
+            assert a[0] == c[0] and (a[0] == 1 or (a[1] > 0, a[2]) == (c[1] > 0, c[2])), (b, a, c)
             b = g.sse_chunk().replace(b"\r\n", b"\n")
-            if not d2(b):
-                a = orklib.parse_sse_chunk(b)
-                rc, usage, _ = hm.parse_sse_chunk_split(b)
-                assert a[0] == rc and (rc == 1 or a[1] == usage), (b, a, rc, usage)
+            a = orklib.parse_sse_chunk(b)
+            rc, usage, _ = hm.parse_sse_chunk_split(b)
+            assert a[0] == rc and (rc == 1 or a[1] == usage), (b, a, rc, usage)
         r = random.Random(5)
         for _ in range(300):
             b = _long_doc(r, "req")
