@@ -173,11 +173,16 @@ int hm_work_profile(int kind, const uint8_t* body, size_t len, uint32_t* advance
 #include <cstdlib>
 #include "../arks_b200/csrc/mask_scan.cuh"
 extern "C" {
-// every call also runs the two-lane form of pass A (fast_scan_host_split): same verdict and same output, or the test dies
+// every call also runs the two-lane form of pass A (fast_scan_host_split): same verdict and same output, or the test dies.
+// One stated exception (fast_esc_after): when the 32 bytes in front of the split point are all backslashes the second lane
+// cannot know its escape carry, and the two-lane form declines a document the one-lane form may accept.
 static void split_must_agree(bool ok, const FastOut& o, bool ok2, const FastOut& o2, const uint8_t* body, size_t len) {
-  const bool same = ok == ok2 && (!ok || (o.m_start == o2.m_start && o.m_rawlen == o2.m_rawlen && o.m_esc == o2.m_esc && o.stream3 == o2.stream3 &&
-                                          o.so_present == o2.so_present && o.iu3 == o2.iu3 && o.usage[0] == o2.usage[0] &&
-                                          o.usage[1] == o2.usage[1] && o.usage[2] == o2.usage[2]));
+  const uint32_t nch = (uint32_t)((len + 31) / 32), h = fast_split_point(nch);
+  bool blind = ok && !ok2 && h && h < nch;
+  for (uint32_t p = 32 * (h - 1); blind && p < 32 * h; p++) blind = body[p] == '\\';
+  const bool same = blind || (ok == ok2 && (!ok || (o.m_start == o2.m_start && o.m_rawlen == o2.m_rawlen && o.m_esc == o2.m_esc && o.stream3 == o2.stream3 &&
+                                                    o.so_present == o2.so_present && o.iu3 == o2.iu3 && o.usage[0] == o2.usage[0] &&
+                                                    o.usage[1] == o2.usage[1] && o.usage[2] == o2.usage[2])));
   if (!same) {
     fprintf(stderr, "split pass A disagrees with the one-lane form (ok %d vs %d) on %zu bytes: %.*s\n", (int)ok, (int)ok2, len, (int)(len < 400 ? len : 400), body);
     abort();
