@@ -2008,6 +2008,7 @@ struct arks_ctx {
   bool ev_meter_set = false;
   bool is_req_timing = false;
   bool last_two_stage = false;
+  int last_route = -1;           // staging route of the last stage_* call (arks_last_staging_route)
   const uint32_t* last_slow_n = nullptr;
   uint8_t* d_inter = nullptr;    // intermediates + group table
   uint32_t* d_perm = nullptr;    // lane -> body permutation of the batch being scanned (length order)
@@ -2233,6 +2234,7 @@ int64_t arks_last_declined(arks_ctx* ctx) {
   return (int64_t)(v + 1u);  // the counter starts at -1
 }
 uint64_t arks_launch_count(const arks_ctx* ctx) { return ctx ? ctx->launches : 0; }
+int arks_last_staging_route(const arks_ctx* ctx) { return ctx ? ctx->last_route : -1; }
 
 int arks_sync_quota_usage(arks_ctx* ctx, int mode, uint32_t* status_present, int64_t* status_used, uint8_t* action) {
   if (!ctx || !ctx->loaded) return ARKS_E_NOT_LOADED;
@@ -2974,6 +2976,9 @@ int arks_last_kernel_ms(arks_ctx* ctx, float* ms, int cap) {
 // ---- request phase ------------------------------------------------------------------------------
 int arks_stage_request_batch(arks_ctx* ctx, const arks_request_batch* b) {
   if (!ctx || !b) return ARKS_E_INVALID_ARG;
+  // a batch that is refused below, for any reason, leaves nothing to run in this slot (not even its previous tenant)
+  ctx->slots[ctx->cur].req_staged = false;
+  ctx->last_route = -1;  // until the bodies are on their way
   if (!ctx->loaded) return fail(ctx, ARKS_E_NOT_LOADED, "arks_load_tables has not been called");
   const uint32_t n = b->n;
   if (n > ctx->max_batch) return fail(ctx, ARKS_E_CAPACITY, "batch of %u exceeds max_batch %u", n, ctx->max_batch);
@@ -2982,7 +2987,6 @@ int arks_stage_request_batch(arks_ctx* ctx, const arks_request_batch* b) {
   int rc = ensure_slot(ctx, ctx->cur, true, false);
   if (rc) return rc;
   arks_ctx::Slot& sl = ctx->slots[ctx->cur];
-  sl.req_staged = false;  // a batch that is refused below leaves nothing to run in this slot
   sl.req_n = n;
   if (n == 0) { sl.req_staged = true; return 0; }
   if (!b->body_off || !b->body_len || !b->token_off || (b->bodies_bytes && !b->bodies) || (b->token_off[n] && !b->tokens))
@@ -3033,6 +3037,7 @@ int arks_stage_request_batch(arks_ctx* ctx, const arks_request_batch* b) {
   r.tokens = sl.d_req_meta + o_tok;
   r.n = n;
   sl.req_staged = true;
+  ctx->last_route = small ? (b->bodies_bytes <= kTinyBatchBytes ? 0 : 1) : 2;
   return 0;
 }
 
@@ -3299,6 +3304,9 @@ static int32_t resolve_qos(const arks_ctx* ctx, int32_t q, uint32_t g) {
 }
 int arks_stage_response_batch(arks_ctx* ctx, const arks_response_batch* b) {
   if (!ctx || !b) return ARKS_E_INVALID_ARG;
+  // a batch that is refused below, for any reason, leaves nothing to run in this slot (not even its previous tenant)
+  ctx->slots[ctx->cur].resp_staged = false;
+  ctx->last_route = -1;  // until the bodies are on their way
   if (!ctx->loaded) return fail(ctx, ARKS_E_NOT_LOADED, "arks_load_tables has not been called");
   const uint32_t n = b->n;
   if (n > ctx->max_batch) return fail(ctx, ARKS_E_CAPACITY, "batch of %u exceeds max_batch %u", n, ctx->max_batch);
@@ -3307,7 +3315,6 @@ int arks_stage_response_batch(arks_ctx* ctx, const arks_response_batch* b) {
   int rc = ensure_slot(ctx, ctx->cur, false, true);
   if (rc) return rc;
   arks_ctx::Slot& sl = ctx->slots[ctx->cur];
-  sl.resp_staged = false;  // a batch that is refused below leaves nothing to run in this slot
   sl.resp_n = n;
   if (n == 0) { sl.resp_staged = true; return 0; }
   if (!b->body_off || !b->body_len || !b->qos || !b->flags || (b->bodies_bytes && !b->bodies)) return fail(ctx, ARKS_E_INVALID_ARG, "response batch: null array");
@@ -3375,6 +3382,7 @@ int arks_stage_response_batch(arks_ctx* ctx, const arks_response_batch* b) {
   r.usage = (long long*)(rb + 2 * align_up(n, 16));
   r.bpe = (uint32_t*)(rb + 2 * align_up(n, 16) + (size_t)n * 24);
   sl.resp_staged = true;
+  ctx->last_route = small ? (b->bodies_bytes <= kTinyBatchBytes ? 0 : 1) : 2;
   return 0;
 }
 

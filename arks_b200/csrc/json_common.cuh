@@ -14,6 +14,13 @@
 #define ARKS_OUTLINE inline
 #endif
 
+// Host drivers of the scan filters (mask_scan.cuh, warp_scan.cuh; tests only): the byte they see at position p >= len of
+// a document, where the device reads whatever the staging buffer holds (the padding, the next body, stale bytes). `dflt`
+// is the driver's own fill; a test defines this to hand over the bytes that follow the body in its buffer instead.
+#ifndef ARKS_HOST_PAST_END
+#define ARKS_HOST_PAST_END(doc, len, p, dflt) (dflt)
+#endif
+
 namespace arks {
 
 enum : uint8_t { K_REQ = 0, K_RESP = 1, K_EVT = 2 };

@@ -686,7 +686,7 @@ inline bool fast_scan_host(const uint8_t* doc, uint32_t len, FastOut& out) {
       uint32_t v = 0;
       for (int b = 0; b < 4; b++) {
         const uint32_t p = 32 * j + 4 * q + b;
-        v |= (uint32_t)(p < len ? doc[p] : (uint8_t)(0xA5 ^ p)) << (8 * b);  // garbage past the end, as on the device
+        v |= (uint32_t)(p < len ? doc[p] : ARKS_HOST_PAST_END(doc, len, p, (uint8_t)(0xA5 ^ p))) << (8 * b);  // garbage past the end, as on the device
       }
       w[q] = v;
     }
@@ -721,7 +721,7 @@ inline bool fast_scan_host_split(const uint8_t* doc, uint32_t len, FastOut& out)
       uint32_t v = 0;
       for (int b = 0; b < 4; b++) {
         const uint32_t p = 32 * j + 4 * q + b;
-        v |= (uint32_t)(p < len ? doc[p] : (uint8_t)(0xA5 ^ p)) << (8 * b);
+        v |= (uint32_t)(p < len ? doc[p] : ARKS_HOST_PAST_END(doc, len, p, (uint8_t)(0xA5 ^ p))) << (8 * b);
       }
       w[q] = v;
     }

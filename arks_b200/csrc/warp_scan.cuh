@@ -522,8 +522,10 @@ inline bool fast_scan_host(const uint8_t* doc, uint32_t len, FastOut& out, uint3
       const uint32_t base = seg * kFastSeg + 32u * l;
       for (int j = 0; j < 8; j++) {
         uint32_t w = 0;
-        for (int b = 0; b < 4; b++)
-          if (base + 4 * j + b < len) w |= (uint32_t)doc[base + 4 * j + b] << (8 * b);
+        for (int b = 0; b < 4; b++) {  // a lane that starts inside the document reads 32 bytes of shared memory, past the end too
+          const uint32_t p = base + 4 * j + b;
+          w |= (uint32_t)(p < len ? doc[p] : base < len ? ARKS_HOST_PAST_END(doc, len, p, (uint8_t)0) : (uint8_t)0) << (8 * b);
+        }
         m[l].w[j] = w;
       }
       fast_masks(m[l], base < len ? (len - base < 32 ? len - base : 32) : 0);

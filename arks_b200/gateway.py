@@ -91,6 +91,8 @@ def lib():
         L.arks_last_declined.argtypes = [vp]
         L.arks_launch_count.restype = C.c_uint64
         L.arks_launch_count.argtypes = [vp]
+        L.arks_last_staging_route.restype = C.c_int
+        L.arks_last_staging_route.argtypes = [vp]
         L.arks_snapshot_quota.argtypes = [vp, abi.i64p]
         L.arks_set_quota_usage.argtypes = [vp, C.c_uint32, abi.i64p]
         L.arks_incr_quota_usage.argtypes = [vp, C.c_uint32, abi.i64p]
@@ -123,7 +125,7 @@ EXPORTED = [  # every symbol include/arks_gateway.h declares (checked by tests/t
     "arks_submit_response_batch", "arks_stage_request_batch", "arks_run_request_batch",
     "arks_fetch_request_result", "arks_stage_response_batch", "arks_run_response_batch",
     "arks_fetch_response_result", "arks_submit_request_async", "arks_wait_request", "arks_submit_response_async",
-    "arks_wait_response", "arks_select_slot", "arks_set_profiling", "arks_last_kernel_ms", "arks_stream", "arks_launch_count", "arks_last_declined", "arks_enable_metrics", "arks_snapshot_metrics", "arks_sync_quota_usage", "arks_alloc_pinned", "arks_free_pinned", "arks_snapshot_quota",
+    "arks_wait_response", "arks_select_slot", "arks_set_profiling", "arks_last_kernel_ms", "arks_stream", "arks_launch_count", "arks_last_declined", "arks_last_staging_route", "arks_enable_metrics", "arks_snapshot_metrics", "arks_sync_quota_usage", "arks_alloc_pinned", "arks_free_pinned", "arks_snapshot_quota",
     "arks_set_quota_usage", "arks_incr_quota_usage", "arks_snapshot_rate", "arks_take_quota_delta",
     "arks_apply_quota_delta", "arks_quota_delta_dev", "arks_fold_quota_delta_dev", "arks_enable_quota_sharing",
     "arks_comm_unique_id", "arks_comm_init", "arks_comm_set_shared", "arks_fold_quota_allreduce", "arks_comm_destroy",
@@ -362,6 +364,12 @@ class Gateway:
     @property
     def launch_count(self) -> int:
         return int(lib().arks_launch_count(self._h))
+
+    @property
+    def last_staging_route(self) -> int:
+        """where the last staged batch's bodies went: 0 the metadata upload (<= 16 KiB), 1 behind the metadata on the compute
+        stream (<= 256 KiB), 2 the slot's bodies buffer; -1 nothing staged (empty or refused batch)"""
+        return int(lib().arks_last_staging_route(self._h))
 
     # ---- quota.QuotaService surface + A14 snapshot
     def snapshot_quota(self) -> np.ndarray:

@@ -151,7 +151,13 @@ typedef struct arks_request_batch {
                                * (32-byte aligned bodies are read a whole sector at a time)      */
   const uint32_t* body_off;   /* n: byte offset of body i (multiple of 16)                      */
   const uint32_t* body_len;   /* n: exact length                                                */
-  uint64_t bodies_bytes;      /* total size of `bodies` (last body padded up to 16)             */
+  uint64_t bodies_bytes;      /* bytes of `bodies` uploaded: must cover body_off[i] + body_len[i] *
+                               * of every body (or the batch is refused), at most max_batch_bytes *
+                               * of arks_create (the library takes up to that + 16, rounded up   *
+                               * to 256). The padding between bodies and whatever follows        *
+                               * bodies_bytes may hold anything: the kernels read past a body's  *
+                               * end and never let those bytes change a result. Same for         *
+                               * arks_response_batch.                                            */
   const uint8_t* tokens;      /* concatenated bearer tokens (output of arks_extract_bearer)     */
   const uint32_t* token_off;  /* n + 1, non-decreasing (a batch that breaks this or the body     *
                                * bounds is refused as a whole: ARKS_E_INVALID_ARG, nothing staged) */
@@ -392,6 +398,11 @@ void* arks_stream(arks_ctx* ctx);
 int64_t arks_last_declined(arks_ctx* ctx);
 /* number of kernel launches issued by this context so far */
 uint64_t arks_launch_count(const arks_ctx* ctx);
+/* how the last arks_stage_* call (also inside the submit calls) placed its bodies in device memory: 0 in the metadata
+ * upload (bodies_bytes <= 16 KiB), 1 behind the metadata on the compute stream (<= 256 KiB and, for requests, room left
+ * behind the metadata and bearer tokens), 2 in the slot's own bodies buffer, uploaded on the copy stream; -1 when that
+ * call staged no bodies (an empty or a refused batch). A diagnostic for tests: results never depend on the route. */
+int arks_last_staging_route(const arks_ctx* ctx);
 
 /* N3 (SURVEY.md §8f): the gateway's Prometheus series that are functions of the request stream
  * (pkg/gateway/metrics/metrics.go:24-98, collector.go:35-53), accumulated on the device next to the counters and read at

@@ -1,7 +1,13 @@
 // host_machine.cpp — TEST-ONLY build of arks_b200/csrc/json_engine.cuh with g++ so the device state
 // machines can be fuzzed against the oracle on CPU (tests/test_machine_vs_oracle.py). Not shipped.
 #include <stddef.h>
+#include <stdint.h>
 #include <string.h>
+
+// Bytes the caller's buffer holds behind the document (hm_set_past_end): the host drivers read them past the end instead
+// of their fixed fills, as the device reads the padding, the next body or stale staging memory there.
+static thread_local size_t g_past = 0;
+#define ARKS_HOST_PAST_END(doc, len, p, dflt) ((size_t)(p) - (size_t)(len) < g_past ? (doc)[p] : (dflt))
 
 #include "../arks_b200/csrc/json_engine.cuh"
 
@@ -11,20 +17,20 @@ using namespace arks;
 
 static int g_evsync = 0;  // schedule for JsonT documents: 0 consume_t, 1 consume_evsync, 4 / 8 consume_rounds<R>
 
-// same bulk loop the kernels run, with units read straight from memory (zero padded past the end)
+// same bulk loop the kernels run, with units read straight from memory; past the end: the `avail` bytes the buffer holds
+// from `body` on, then a fixed fill
 template <class M>
-static void feed(M& m, const uint8_t* body, size_t len, uint32_t begin = 0) {
+static void feed(M& m, const uint8_t* body, size_t len, uint32_t begin = 0, size_t avail = (size_t)-1) {
+  if (avail == (size_t)-1) avail = len + g_past;
   uint32_t pos = begin;
   // exercise window boundaries like the tiled kernels do: consume in 128-byte windows
   for (uint32_t wbeg = 0; wbeg < len; wbeg += 128) {
     uint32_t lim = (uint32_t)(len < wbeg + 128 ? len : wbeg + 128);
     auto load = [&](uint32_t u) {
       Unit16 q;
-      uint8_t tmp[16] = {0};
-      size_t o = (size_t)u * 16;
-      size_t n = o < len ? (len - o < 16 ? len - o : 16) : 0;
-      memcpy(tmp, body + o, n);
-      for (int k = 0; k < 16; k++) tmp[k] = k < (int)n ? tmp[k] : (uint8_t)(0xA5 ^ k);  // garbage past the end
+      uint8_t tmp[16];
+      const size_t o = (size_t)u * 16;
+      for (int k = 0; k < 16; k++) tmp[k] = o + k < avail ? body[o + k] : (uint8_t)(0xA5 ^ k);  // garbage past the end
       memcpy(q.w, tmp, 16);
       return q;
     };
@@ -42,6 +48,7 @@ static void feed(M& m, const uint8_t* body, size_t len, uint32_t begin = 0) {
 
 extern "C" {
 void hm_set_evsync(int on) { g_evsync = on; }
+void hm_set_past_end(size_t n) { g_past = n; }
 int hm_parse_request(const uint8_t* body, size_t len, uint8_t* model_out, size_t cap, size_t* model_len, int* stream,
                      int* so_present, int* iu) {
   static thread_local JsonT m;
@@ -100,7 +107,8 @@ int hm_parse_sse_split(const uint8_t* body, size_t len, int64_t usage[3]) {
   for (size_t ub = 0; ub < len; ub += 16) {
     uint8_t tmp[16];
     size_t n = len - ub < 16 ? len - ub : 16;
-    for (int k = 0; k < 16; k++) tmp[k] = k < (int)n ? body[ub + k] : (uint8_t)(0x0a ^ (k & 1 ? 0x07 : 0));  // hostile padding: LF / CR
+    for (int k = 0; k < 16; k++)  // past the end: the caller's bytes, then hostile padding: LF / CR
+      tmp[k] = ub + k < len + g_past ? body[ub + k] : (uint8_t)(0x0a ^ (k & 1 ? 0x07 : 0));
     uint32_t q[4];
     memcpy(q, tmp, 16);
     sp.unit((uint32_t)ub, (uint32_t)n, q[0], q[1], q[2], q[3], [&](uint32_t off, uint32_t l) {
@@ -116,7 +124,7 @@ int hm_parse_sse_split(const uint8_t* body, size_t len, int64_t usage[3]) {
     const uint32_t begin = offs[e] & 15u, end = begin + lens[e];
     JsonT m;
     m.init(K_EVT, base, stk, &cold, host_json_tables());
-    feed(m, base, end, begin);
+    feed(m, base, end, begin, len + g_past - (offs[e] & ~15u));
     SseEventVerdict v = sse_event_verdict(m, end);
     if (v.fail) fail = true;
     else if (v.no_choices) for (int k = 0; k < 3; k++) usage[k] = cold.usage[k];

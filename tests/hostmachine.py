@@ -37,6 +37,7 @@ def lib():
         L.hm_bpe_count.argtypes = [C.c_char_p, C.c_size_t]
         L.hm_bpe_count.restype = C.c_uint32
         L.hm_bpe_pretokenize.argtypes = [C.c_char_p, C.c_size_t, u32p, C.c_int]
+        L.hm_set_past_end.argtypes = [C.c_size_t]
         L.hm_work_profile.argtypes = [C.c_int, C.c_char_p, C.c_size_t, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.c_size_t]
         vp, cp, u32 = C.c_void_p, C.c_char_p, C.c_uint32
         L.hm_store_new.restype = vp
@@ -53,30 +54,37 @@ def lib():
     return _lib
 
 
-def parse_request_body(body: bytes):
+def _past(body: bytes, past: bytes) -> bytes:
+    """the buffer a host driver is handed: the document, then `past`, the bytes it finds behind the document's end (the
+    device reads the padding, the next body or stale staging memory there); without `past`, the drivers' fixed fills"""
+    lib().hm_set_past_end(len(past))
+    return body + past
+
+
+def parse_request_body(body: bytes, past: bytes = b""):
     buf = C.create_string_buffer(4096)
     ml, st, so, iu = C.c_size_t(), C.c_int(), C.c_int(), C.c_int()
-    rc = lib().hm_parse_request(body, len(body), buf, 4096, C.byref(ml), C.byref(st), C.byref(so), C.byref(iu))
+    rc = lib().hm_parse_request(_past(body, past), len(body), buf, 4096, C.byref(ml), C.byref(st), C.byref(so), C.byref(iu))
     return rc, buf.raw[:min(ml.value, 4096)], st.value, so.value, iu.value
 
 
-def parse_response_body(body: bytes):
+def parse_response_body(body: bytes, past: bytes = b""):
     ne = C.c_size_t()
     u = np.zeros(3, np.int64)
-    rc = lib().hm_parse_response(body, len(body), C.byref(ne), u.ctypes.data_as(C.POINTER(C.c_int64)))
+    rc = lib().hm_parse_response(_past(body, past), len(body), C.byref(ne), u.ctypes.data_as(C.POINTER(C.c_int64)))
     return rc, ne.value, tuple(int(x) for x in u)
 
 
-def parse_sse_chunk(body: bytes):
+def parse_sse_chunk(body: bytes, past: bytes = b""):
     u = np.zeros(3, np.int64)
-    rc = lib().hm_parse_sse(body, len(body), u.ctypes.data_as(C.POINTER(C.c_int64)))
+    rc = lib().hm_parse_sse(_past(body, past), len(body), u.ctypes.data_as(C.POINTER(C.c_int64)))
     return rc, tuple(int(x) for x in u)
 
 
-def parse_sse_chunk_split(body: bytes):
+def parse_sse_chunk_split(body: bytes, past: bytes = b""):
     """the event-parallel path of the SSE kernel (SseSplit + one JsonT per event); third item: fell back to SseT"""
     u = np.zeros(3, np.int64)
-    rc = lib().hm_parse_sse_split(body, len(body), u.ctypes.data_as(C.POINTER(C.c_int64)))
+    rc = lib().hm_parse_sse_split(_past(body, past), len(body), u.ctypes.data_as(C.POINTER(C.c_int64)))
     return rc & 1, tuple(int(x) for x in u), bool(rc & 2)
 
 
@@ -96,37 +104,37 @@ def work_profile(body: bytes, kind: int = 0):
     return a[:n], e[:n]
 
 
-def _req(fn, body):
+def _req(fn, body, past):
     span = (C.c_uint32 * 3)()
     st, so, iu = C.c_int(), C.c_int(), C.c_int()
-    ok = fn(body, len(body), span, C.byref(st), C.byref(so), C.byref(iu))
+    ok = fn(_past(body, past), len(body), span, C.byref(st), C.byref(so), C.byref(iu))
     return (tuple(span), st.value, so.value, iu.value) if ok else None
 
 
-def _resp(fn, body):
+def _resp(fn, body, past):
     span = (C.c_uint32 * 3)()
     u = (C.c_int64 * 3)()
-    ok = fn(body, len(body), span, u)
+    ok = fn(_past(body, past), len(body), span, u)
     return (tuple(span), tuple(u)) if ok else None
 
 
-def fast_request(body: bytes):
+def fast_request(body: bytes, past: bytes = b""):
     """the fast path (host driver of mask_scan.cuh = one lane's work): ((start, rawlen, esc), stream3, so_present, iu3) or
     None when the document is left to the exact engine"""
-    return _req(lib().hm_fast_request, body)
+    return _req(lib().hm_fast_request, body, past)
 
 
-def engine_request(body: bytes):
+def engine_request(body: bytes, past: bytes = b""):
     """the exact engine in the same terms, None when it rejects the document"""
-    return _req(lib().hm_engine_request_span, body)
+    return _req(lib().hm_engine_request_span, body, past)
 
 
-def fast_response(body: bytes):
-    return _resp(lib().hm_fast_response, body)
+def fast_response(body: bytes, past: bytes = b""):
+    return _resp(lib().hm_fast_response, body, past)
 
 
-def engine_response(body: bytes):
-    return _resp(lib().hm_engine_response_span, body)
+def engine_response(body: bytes, past: bytes = b""):
+    return _resp(lib().hm_engine_response_span, body, past)
 
 
 def bpe_load(tables):
@@ -149,8 +157,8 @@ def bpe_probes():
     return [int(x) for x in out]
 
 
-def bpe_count(body: bytes) -> int:
-    return int(lib().hm_bpe_count(body, len(body)))
+def bpe_count(body: bytes, past: bytes = b"") -> int:
+    return int(lib().hm_bpe_count(_past(body, past), len(body)))
 
 
 def bpe_pretokenize(text: bytes):
@@ -160,13 +168,13 @@ def bpe_pretokenize(text: bytes):
     return list(ends[:n])
 
 
-def warp_request(body: bytes):
+def warp_request(body: bytes, past: bytes = b""):
     """the warp-per-document latency path (host driver of warp_scan.cuh), same convention as fast_request"""
-    return _req(lib().hm_warp_request, body)
+    return _req(lib().hm_warp_request, body, past)
 
 
-def warp_response(body: bytes):
-    return _resp(lib().hm_warp_response, body)
+def warp_response(body: bytes, past: bytes = b""):
+    return _resp(lib().hm_warp_response, body, past)
 
 
 class ConfigStore:
