@@ -49,7 +49,21 @@ def parse_args(argv=None):
                    help="charge admitted requests' BPE counts to tpm / tpd at request time (needs --bpe.tokenizer)")
     p.add_argument("--bpe.stream-metering", dest="bpe_stream_metering", action="store_true",
                    help="decide and bill streams without stream_options.include_usage by their BPE counts (needs --bpe.tokenizer)")
+    p.add_argument("--gateway.ratelimit-headers", dest="ratelimit_headers", action="store_true",
+                   help="send x-ratelimit-{limit,remaining,reset}-{requests,tokens} on every decided request and retry-after on "
+                        "rate-limit 429s (off by default: the reference sends none)")
     return p.parse_args(argv)
+
+
+def configure_ratelimit_headers(engine, batcher, args):
+    """--gateway.ratelimit-headers as library calls, made before the first generation is published: the rate-limit report of
+    the context (arks_set_ratelimit_report), through the compiled batcher when there is one (its stream state machine shapes
+    the headers). Without the flag: no call at all."""
+    if not args.ratelimit_headers:
+        return
+    if batcher is not None:
+        batcher.b.set_ratelimit_report(True)
+    engine.set_ratelimit_report(True)
 
 
 def configure_bpe(engine, args, load=None):
@@ -219,6 +233,7 @@ def main(argv=None) -> int:
     if args.batcher == "compiled":
         batcher = extproc.CompiledBatcher(cpphost.Batcher(cpphost.load(cpphost.build()), g._h, max_batch=args.max_batch,
                                                           max_bytes=args.max_bytes))
+    configure_ratelimit_headers(g, batcher, args)  # before Assembly.start() publishes the first generation
     status_out = None if args.status_out == "-" else open(args.status_out, "a")
     asm = Assembly(g, args, batcher=batcher, status_out=status_out).start()
     print(f"arks_b200 gateway: gRPC :{asm.grpc_port}, http :{asm.http_port}, metrics :{asm.metrics_port}, device {args.device}, "

@@ -141,6 +141,11 @@ struct ReqDev {  // request batch, device resident
   uint32_t* bpe;        // BPE tokens of the prompt text (0 without a vocabulary)
   int precharge;  // N4: admitted requests charge their BPE count to the token-type rules
   int meter;      // N5: stream requests without include_usage are decided and metered instead of refused
+  // rate-limit report (arks_set_ratelimit_report), 2n each: [2i] the requests figure, [2i + 1] the tokens figure. All three
+  // null when the report is off
+  uint8_t* rl_entry;
+  long long* rl_limit;
+  long long* rl_remaining;  // last: the scan kernels' parameter offsets stay as they were
 };
 
 struct RespDev {
@@ -1247,14 +1252,18 @@ __global__ void __launch_bounds__(128) limit_admit_kernel(DevTables T, ReqDev B)
     }
     if (qt == ARKS_QUOTA_MISSING || quota_fail >= 0) k = 0;
   }
-  // ---- phase B: arrival rank inside the group, only for groups that straddle their limit (0 < k < n_g)
-  const bool need_rank = slot >= 0 && k > 0 && k < n_g;
+  // ---- phase B: arrival rank inside the group, only for groups that straddle their limit (0 < k < n_g); with the rate-limit
+  // report on, for every group with admissions (an admitted row reports the counters as of its own admission)
+  const bool report = B.rl_entry != nullptr;
+  const bool need_rank = slot >= 0 && k > 0 && (k < n_g || report);
   long long rank = 0;
   if (need_rank && n_g <= kHotGroup) {  // small group: walk its member list
     for (int32_t j = B.ghead[slot]; j >= 0; j = B.gnext[j]) rank += (uint32_t)j < i;
   }
   if (need_rank && n_g > kHotGroup) rank = B.hotrank[i];  // hot tenant: ranked by rank_hot_groups_kernel
   // ---- phase C: decision, commit, pick
+  uint8_t rq_e = 0xFF, tk_e = 0xFF;  // rate-limit report: the requests figure and the tokens figure (scalars: no local memory)
+  long long rq_lim = 0, rq_rem = 0, tk_lim = 0, tk_rem = 0;
   if (slot >= 0) {
     const bool admitted = k >= n_g ? true : k <= 0 ? false : rank < k;
     if (!admitted) {
@@ -1274,6 +1283,20 @@ __global__ void __launch_bounds__(128) limit_admit_kernel(DevTables T, ReqDev B)
       if (!reason) {
         if (qt == ARKS_QUOTA_MISSING) reason = ARKS_R_QUOTA_CONFIG;
         else { reason = ARKS_R_QUOTA; detail = (uint8_t)quota_fail; cur_out = q_cur; lim_out = q_lim; }
+      }
+    }
+    // rate-limit report: the counters as the serial order leaves them right after this row, a = admissions of the group up to
+    // and including it (rank + 1 if admitted, all k otherwise); token-type counters as of the batch's start. Per kind the
+    // entry with the least room, the first one on a tie
+    if (report && reason != ARKS_R_QUOTA_CONFIG) {
+      const long long a = admitted ? rank + 1 : k;
+      for (uint32_t j = rl0; j < rl1; j++) {
+        const int rule = T.rl_rule[j];
+        const long long lim = T.rl_value[j];
+        const long long c = rule < 2 ? cur[rule] + a * cnt[rule] : cur[rule];
+        const long long rem = c >= lim ? 0 : lim - c;
+        if (rule < 2 && (rq_e == 0xFF || rem < rq_rem)) { rq_e = (uint8_t)(j - rl0); rq_lim = lim; rq_rem = rem; }
+        if (rule >= 2 && (tk_e == 0xFF || rem < tk_rem)) { tk_e = (uint8_t)(j - rl0); tk_lim = lim; tk_rem = rem; }
       }
     }
     // N4 (opt-in): the estimate is charged when the micro-batch commits; nobody reads T.rate here. Metered rows (N5) are
@@ -1313,6 +1336,11 @@ __global__ void __launch_bounds__(128) limit_admit_kernel(DevTables T, ReqDev B)
   B.pick[i] = pick;
   B.cur_usage[i] = cur_out;
   B.limit_max[i] = lim_out;
+  if (report) {
+    reinterpret_cast<uchar2*>(B.rl_entry)[i] = make_uchar2(rq_e, tk_e);
+    reinterpret_cast<longlong2*>(B.rl_limit)[i] = make_longlong2(rq_lim, tk_lim);
+    reinterpret_cast<longlong2*>(B.rl_remaining)[i] = make_longlong2(rq_rem, tk_rem);
+  }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1923,6 +1951,7 @@ struct arks_ctx {
   std::mutex cfg_mu;                  // prepare (config thread) vs commit (batch thread)
   bool precharge = false;              // N4 (arks_set_precharge)
   bool meter = false;                  // N5 (arks_set_stream_metering)
+  bool rl_report = false;              // arks_set_ratelimit_report
   bool split = false;                  // fast path: two lanes per document in pass A (fast_*_kernel2), ARKS_SPLIT=1; measured slower
   bool walk8 = true;                   // fast path, pass B: the step inlined eight times (true) or one copy in a loop
   int regroup = 1;                     // fast path: regroup a block's documents by structure between passes A and B
@@ -1978,6 +2007,7 @@ struct arks_ctx {
     cudaEvent_t req_done = nullptr, resp_done = nullptr;
     cudaEvent_t req_ran = nullptr, resp_ran = nullptr;  // the slot's device buffers are free again (kernels done)
     uint32_t req_fetch_n = 0, resp_fetch_n = 0;
+    bool req_report = false;  // the request batch in this slot was run with the rate-limit report (its result block is longer)
     ReqDev rq{};
     RespDev rp{};
     uint32_t req_n = 0, resp_n = 0;
@@ -2160,7 +2190,8 @@ int arks_create(int device, uint32_t max_batch, uint64_t max_batch_bytes, arks_c
   CK(cudaMalloc(&ctx->d_slow, (size_t)4 * max_batch + 256));
 
   CK(cudaMalloc(&ctx->d_lenhist, (size_t)4 * kLenBuckets));
-  ctx->result_cap = align_up(n, 256) * 3 + align_up(n * 4, 256) * 6 + align_up(n * 8, 256) * 3;
+  ctx->result_cap = align_up(n, 256) * 3 + align_up(n * 4, 256) * 6 + align_up(n * 8, 256) * 3 +
+                    align_up(n * 2, 256) + align_up(n * 16, 256) * 2;  // + the rate-limit report's three arrays
   CK(cudaMalloc(&ctx->d_result, ctx->result_cap));
   CK(cudaMemset(ctx->d_result, 0, ctx->result_cap));  // the packed block has alignment gaps that the D2H copies too
   return 0;
@@ -2877,6 +2908,11 @@ int arks_set_precharge(arks_ctx* ctx, int on) {
   ctx->precharge = on != 0;
   return 0;
 }
+int arks_set_ratelimit_report(arks_ctx* ctx, int on) {
+  if (!ctx) return ARKS_E_INVALID_ARG;
+  ctx->rl_report = on != 0;
+  return 0;
+}
 int arks_set_stream_metering(arks_ctx* ctx, int on) {
   if (!ctx) return ARKS_E_INVALID_ARG;
   if (on && !ctx->bpe_on) return fail(ctx, ARKS_E_NOT_LOADED, "stream metering needs a vocabulary (arks_load_bpe)");
@@ -3041,18 +3077,22 @@ int arks_stage_request_batch(arks_ctx* ctx, const arks_request_batch* b) {
   return 0;
 }
 
-// offsets of the 11 result arrays inside the packed result block of a batch of n (dense: one D2H for any n)
-constexpr int kReqResultArrays = 11;
-static void result_offsets(size_t n, size_t offs[kReqResultArrays + 1]) {
+// offsets of the 11 result arrays inside the packed result block of a batch of n (dense: one D2H for any n), and with the
+// rate-limit report 3 more behind them (rl_entry 2n bytes, rl_limit and rl_remaining 2n int64). Returns the block's size
+constexpr int kReqResultArrays = 11, kReqReportArrays = 3;
+static size_t result_offsets(size_t n, bool report, size_t offs[kReqResultArrays + kReqReportArrays + 1]) {
   const size_t a1 = align_up(n, 16), a4 = align_up(n * 4, 16), a8 = align_up(n * 8, 16);
   offs[0] = 0; offs[1] = a1; offs[2] = 2 * a1; offs[3] = 3 * a1; offs[4] = offs[3] + a4; offs[5] = offs[4] + a4;
   offs[6] = offs[5] + a4; offs[7] = offs[6] + a8; offs[8] = offs[7] + a8;
   offs[9] = offs[8] + a4; offs[10] = offs[9] + a4; offs[11] = offs[10] + a4;
+  if (!report) return offs[kReqResultArrays];
+  offs[12] = offs[11] + align_up(n * 2, 16); offs[13] = offs[12] + align_up(n * 16, 16); offs[14] = offs[13] + align_up(n * 16, 16);
+  return offs[kReqResultArrays + kReqReportArrays];
 }
 // Micro-batches write their result rows straight into the slot's pinned host block (zero copy over PCIe: the block is
 // device-addressable under unified addressing): no D2H copy node between the last kernel and the host's wake-up.
 constexpr uint32_t kZeroCopyRows = 2048;
-static void carve_request(arks_ctx* ctx, ReqDev& r, size_t batch_n, uint8_t* result_base) {
+static void carve_request(arks_ctx* ctx, ReqDev& r, size_t batch_n, bool report, uint8_t* result_base) {
   const size_t n = ctx->max_batch;
   uint8_t* p = ctx->d_inter;
   r.st_reason = p; p += align_up(n, 256);
@@ -3068,8 +3108,8 @@ static void carve_request(arks_ctx* ctx, ReqDev& r, size_t batch_n, uint8_t* res
   r.hot_n = (int32_t*)p; p += 256;
   r.hot_list = (int32_t*)p; p += align_up((n / kHotGroup + 2) * 4, 256);
   r.hotrank = (int32_t*)p;
-  size_t offs[kReqResultArrays + 1];
-  result_offsets(batch_n, offs);
+  size_t offs[kReqResultArrays + kReqReportArrays + 1];
+  result_offsets(batch_n, report, offs);
   uint8_t* q = result_base;
   r.reason = q + offs[0];
   r.detail = q + offs[1];
@@ -3082,6 +3122,9 @@ static void carve_request(arks_ctx* ctx, ReqDev& r, size_t batch_n, uint8_t* res
   r.model_off = (uint32_t*)(q + offs[8]);
   r.model_len = (uint32_t*)(q + offs[9]);
   r.bpe = (uint32_t*)(q + offs[10]);
+  r.rl_entry = report ? q + offs[11] : nullptr;
+  r.rl_limit = report ? (long long*)(q + offs[12]) : nullptr;
+  r.rl_remaining = report ? (long long*)(q + offs[13]) : nullptr;
 }
 
 // A warp is as slow as its slowest body and pays for every code path any of its lanes takes, so a small batch is spread
@@ -3128,7 +3171,8 @@ int arks_run_request_batch(arks_ctx* ctx, int64_t now_unix) {
   CK(cudaStreamWaitEvent(ctx->stream, sl.req_copied, 0));
   ReqDev& r = sl.rq;
   sl.req_zc = n <= kZeroCopyRows && sl.h_req_result;
-  carve_request(ctx, r, n, sl.req_zc ? sl.h_req_result : ctx->d_result);
+  sl.req_report = ctx->rl_report;
+  carve_request(ctx, r, n, sl.req_report, sl.req_zc ? sl.h_req_result : ctx->d_result);
   r.meter = ctx->meter ? 1 : 0;
   // batch-local group table sized to the batch (2x, power of two); the three arrays are contiguous
   uint32_t g = 64;
@@ -3218,9 +3262,9 @@ static int enqueue_request_fetch(arks_ctx* ctx) {
   const size_t n = ctx->fetch_n;
   sl.req_fetch_n = (uint32_t)n;
   if (n == 0) return 0;
-  size_t offs[kReqResultArrays + 1];
-  result_offsets(n, offs);
-  if (!sl.req_zc) CK(cudaMemcpyAsync(sl.h_req_result, ctx->d_result, offs[kReqResultArrays], cudaMemcpyDeviceToHost, ctx->stream));
+  size_t offs[kReqResultArrays + kReqReportArrays + 1];
+  const size_t bytes = result_offsets(n, sl.req_report, offs);
+  if (!sl.req_zc) CK(cudaMemcpyAsync(sl.h_req_result, ctx->d_result, bytes, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaEventRecord(sl.req_done, ctx->stream));
   return 0;
 }
@@ -3242,8 +3286,8 @@ static int finish_request_fetch(arks_ctx* ctx, int slot, arks_request_result* ou
   if (n == 0) return 0;
   CK(wait_event_polling(sl.req_done));
   const uint8_t* h = sl.h_req_result;
-  size_t offs[kReqResultArrays + 1];
-  result_offsets(n, offs);
+  size_t offs[kReqResultArrays + kReqReportArrays + 1];
+  result_offsets(n, sl.req_report, offs);
   memcpy(out->reason, h + offs[0], n);
   memcpy(out->detail, h + offs[1], n);
   memcpy(out->flags, h + offs[2], n);
@@ -3255,6 +3299,11 @@ static int finish_request_fetch(arks_ctx* ctx, int slot, arks_request_result* ou
   if (out->model_off) memcpy(out->model_off, h + offs[8], n * 4);
   if (out->model_len) memcpy(out->model_len, h + offs[9], n * 4);
   if (out->bpe_count) memcpy(out->bpe_count, h + offs[10], n * 4);
+  if (sl.req_report) {  // a batch run without the report leaves the caller's arrays untouched
+    if (out->rl_entry) memcpy(out->rl_entry, h + offs[11], n * 2);
+    if (out->rl_limit) memcpy(out->rl_limit, h + offs[12], n * 16);
+    if (out->rl_remaining) memcpy(out->rl_remaining, h + offs[13], n * 16);
+  }
   return 0;
 }
 int arks_fetch_request_result(arks_ctx* ctx, arks_request_result* out) {

@@ -342,6 +342,7 @@ class Batcher:
                 RequestBatch.from_lists([i["body"] for i in reqs], [i["token"] for i in reqs], now, pick_rand=rnd))
             for k, i in enumerate(reqs):
                 i["out"] = {f: v[k] for f, v in r.fields().items()}
+                i["out"].update({f: tuple(v[k]) for f, v in r.report().items()})  # with the rate-limit report on
                 i["out"].update(now=now, gen=gen)
                 i["ev"].set()
         if resps:
@@ -382,7 +383,8 @@ class CompiledBatcher:
         d = self.b.request(token, body, 0)
         return {"reason": d.reason, "detail": d.detail, "flags": d.flags, "qos": d.qos, "token": d.token, "pick": d.pick,
                 "cur_usage": d.cur_usage, "limit_max": d.limit_max, "now": d.now_unix, "gen": d.gen,
-                "model_off": d.model_off, "model_len": d.model_len}
+                "model_off": d.model_off, "model_len": d.model_len, "rl_entry": tuple(d.rl_entry), "rl_limit": tuple(d.rl_limit),
+                "rl_remaining": tuple(d.rl_remaining)}
 
     def response(self, body: bytes, qos: int, flags: int, gen: int = None):
         d = self.b.response(qos, body, flags, gen)
@@ -407,7 +409,7 @@ class ExtProcServer:
 
     # ---- Server.Process, gateway.go:77-138
     def Process(self, request_iterator, context):
-        token, qos, stream, status = b"", (-1, None), False, 0
+        token, qos, stream, status, rl = b"", (-1, None), False, 0, []
         buffered = bytearray()
         start, completed, resp_spent = self.monotonic(), False, 0.0
         for req in request_iterator:
@@ -416,9 +418,9 @@ class ExtProcServer:
                 start = self.monotonic()  # requestStart, gateway.go:108
                 resp, token = self.handle_request_headers(req)
             elif kind == "request_body":
-                resp, qos, stream = self.handle_request_body(req, token)
+                resp, qos, stream, rl = self.handle_request_body(req, token)
             elif kind == "response_headers":
-                resp, status = self.handle_response_headers(req)
+                resp, status = self.handle_response_headers(req, rl)
                 if status == 500:  # gateway.go:115-121 -> responseErrorProcessing keeps the reply's headers, empty message
                     self._record_request(qos, start, status)
                     hs = [(o.header.key, o.header.raw_value) for o in resp.response_headers.response.header_mutation.set_headers]
@@ -492,16 +494,21 @@ class ExtProcServer:
 
     # ---- HandleRequestBody, handle_request.go:83-249 (decision comes from the engine)
     def handle_request_body(self, req, token):
+        """-> (reply, (qos, gen), RESP_* flags of the stream's chunks, rate-limit headers for the response headers)"""
         body = bytes(req.request_body.body)
         out = self.batcher.request(body, token)
         reason = int(out["reason"])
+        rl = replies.ratelimit_headers(reason, int(out["detail"]), int(out["qos"]), int(out.get("now", 0)), out.get("rl_entry"),
+                                       out.get("rl_limit"), out.get("rl_remaining"), self.names_of(out.get("gen")))
         if reason != abi.R_OK:
             ml = int(out.get("model_len", 0))
             raw = body[int(out.get("model_off", 0)):int(out.get("model_off", 0)) + (ml & 0x7FFFFFFF)]
             st, h, v, m = replies.request_error_reply(reason, int(out["detail"]), int(out["cur_usage"]), int(out["limit_max"]),
                                                       int(out.get("now", 0)), self.names_of(out.get("gen")), int(out["qos"]), token,
                                                       replies.decode_model(raw, bool(ml >> 31)))
-            return error_response(st, h, v, m), (-1, None), False
+            r = error_response(st, h, v, m)
+            r.immediate_response.headers.MergeFrom(_set_headers(rl))  # behind x-error-* and Content-Type
+            return r, (-1, None), False, []
         t = self.names_of(out.get("gen"))
         q, tok = int(out["qos"]), int(out["token"])
         r = PB["ProcessingResponse"]()
@@ -509,10 +516,12 @@ class ExtProcServer:
             ("model", t.qos_model_name[q]), ("namespace", t.token_namespace[tok]), ("username", t.token_user[tok])]))
         # a stream's response flags: RESP_METERED rides on every chunk of a stream admitted with FLAG_METERED (N5)
         fl = int(out["flags"])
-        return r, (q, out.get("gen")), (abi.RESP_STREAM | (abi.RESP_METERED if fl & abi.FLAG_METERED else 0)) if fl & 1 else 0
+        return r, (q, out.get("gen")), (abi.RESP_STREAM | (abi.RESP_METERED if fl & abi.FLAG_METERED else 0)) if fl & 1 else 0, rl
 
     # ---- HandleResponseHeaders, handle_response.go:37-78
-    def handle_response_headers(self, req):
+    def handle_response_headers(self, req, rl=()):
+        """`rl`: the stream's rate-limit headers (handle_request_body). They replace any upstream header of the same name,
+        except on an upstream 500, whose reply keeps the reference's headers"""
         pairs, status = [(H_WENT_RESP, "true")], 0
         for h in req.response_headers.headers.headers:
             v = h.raw_value or h.value.encode()
@@ -522,6 +531,9 @@ class ExtProcServer:
                 except ValueError:
                     status = 0
             pairs.append((h.key, v))
+        if rl and status != 500:
+            ours = {k for k, _ in rl}
+            pairs = [(k, v) for k, v in pairs if k.lower() not in ours] + list(rl)
         r = PB["ProcessingResponse"]()
         r.response_headers.response.header_mutation.CopyFrom(_set_headers(pairs))
         r.response_headers.response.clear_route_cache = True

@@ -67,6 +67,7 @@ def lib():
         L.arks_find_qos.restype = C.c_int32
         L.arks_set_precharge.argtypes = [vp, C.c_int]
         L.arks_set_stream_metering.argtypes = [vp, C.c_int]
+        L.arks_set_ratelimit_report.argtypes = [vp, C.c_int]
         L.arks_table_generation.restype = C.c_uint32
         L.arks_table_generation.argtypes = [vp]
         L.arks_update_endpoint_weights.argtypes = [vp, C.c_uint32, C.c_uint32, abi.i32p]
@@ -118,7 +119,7 @@ def lib():
 
 EXPORTED = [  # every symbol include/arks_gateway.h declares (checked by tests/test_abi.py)
     "arks_abi_version", "arks_create", "arks_destroy", "arks_last_error", "arks_load_tables", "arks_table_generation", "arks_load_bpe", "arks_set_precharge",
-    "arks_set_stream_metering", "arks_load_bpe_vocab", "arks_bind_model_vocab",
+    "arks_set_stream_metering", "arks_set_ratelimit_report", "arks_load_bpe_vocab", "arks_bind_model_vocab",
     "arks_prepare_tables", "arks_commit_tables", "arks_discard_prepared", "arks_upsert_token", "arks_delete_token", "arks_upsert_quota",
     "arks_delete_quota", "arks_upsert_endpoint", "arks_delete_endpoint", "arks_config_prepare", "arks_find_quota", "arks_find_qos",
     "arks_update_endpoint_weights", "arks_extract_bearer", "arks_submit_request_batch",
@@ -149,6 +150,7 @@ class Gateway:
                 lib().arks_destroy(h)
             raise ArksError(rc, msg)
         self.tables = None
+        self.ratelimit_report = False
 
     def close(self):
         if getattr(self, "_h", None):
@@ -268,6 +270,12 @@ class Gateway:
         Needs load_bpe"""
         self._ck(lib().arks_set_stream_metering(self._h, int(bool(on))))
 
+    def set_ratelimit_report(self, on: bool):
+        """opt-in: request results carry each row's rate-limit figures (rl_entry / rl_limit / rl_remaining, [n, 2]: requests,
+        tokens) for the x-ratelimit-* and retry-after headers; decisions and counters do not change"""
+        self._ck(lib().arks_set_ratelimit_report(self._h, int(bool(on))))
+        self.ratelimit_report = bool(on)
+
     @property
     def generation(self) -> int:
         """table generation the qos / token indices of request results refer to (carry it with the stream)"""
@@ -279,7 +287,7 @@ class Gateway:
 
     # ---- HandleRequestBody for a micro-batch of streams
     def handle_request_body(self, b: RequestBatch, out: RequestResult | None = None) -> RequestResult:
-        r = out if out is not None else RequestResult.empty(b.n)
+        r = out if out is not None else RequestResult.empty(b.n, self.ratelimit_report)
         bs, rs = b.c_struct(), r.c_struct()
         self._ck(lib().arks_submit_request_batch(self._h, C.byref(bs), C.byref(rs)))
         return r
@@ -319,7 +327,7 @@ class Gateway:
         self._ck(lib().arks_run_request_batch(self._h, int(now_unix)))
 
     def fetch_request(self, n: int, out: RequestResult | None = None) -> RequestResult:
-        r = out if out is not None else RequestResult.empty(n)
+        r = out if out is not None else RequestResult.empty(n, self.ratelimit_report)
         rs = r.c_struct()
         self._ck(lib().arks_fetch_request_result(self._h, C.byref(rs)))
         return r

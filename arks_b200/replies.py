@@ -85,6 +85,41 @@ def decode_model(raw: bytes, escaped: bool) -> str:
     return bytes(o).decode("utf-8", "surrogateescape")
 
 
+def window_end(now_unix: int, rule: str) -> int:
+    """end of the fixed window of `rule` that holds now_unix: the 429 body's expiresAt and the x-ratelimit-reset-* /
+    retry-after headers. Go truncates time relative to year 1 (62135596800 s before the epoch)."""
+    w = WINDOW[rule]
+    return now_unix - ((now_unix + 62135596800) % w) + w
+
+
+def go_duration(seconds: int) -> str:
+    """time.Duration.String() of whole seconds: "1s", "59s", "1m0s", "23h59m59s" (the x-ratelimit-reset-* format)"""
+    h, m, s = seconds // 3600, seconds // 60 % 60, seconds % 60
+    return f"{h}h{m}m{s}s" if h else f"{m}m{s}s" if m else f"{s}s"
+
+
+RATELIMIT_HEADERS = tuple(f"x-ratelimit-{w}-{k}" for k in ("requests", "tokens") for w in ("limit", "remaining", "reset"))
+
+
+def ratelimit_headers(reason: int, detail: int, qos: int, now_unix: int, rl_entry, rl_limit, rl_remaining, tables):
+    """the headers of the rate-limit report (arks_set_ratelimit_report) for one request decision, in wire order: retry-after
+    on a rate-limit 429 (until the denying entry's window ends), then limit / remaining / reset of the requests figure, then
+    of the tokens figure. A figure without an entry (abi.RL_NONE) adds nothing; [] when the decision carries no report."""
+    if reason not in (abi.R_OK, abi.R_RATE_LIMIT, abi.R_QUOTA) or rl_entry is None or all(int(e) == abi.RL_NONE for e in rl_entry):
+        return []
+    names = tables.qos_rule_names[qos]
+    out = []
+    if reason == abi.R_RATE_LIMIT:
+        out.append(("retry-after", str(window_end(now_unix, names[detail]) - now_unix)))
+    for t, kind in enumerate(("requests", "tokens")):
+        e = int(rl_entry[t])
+        if e == abi.RL_NONE:
+            continue
+        out += [(f"x-ratelimit-limit-{kind}", str(int(rl_limit[t]))), (f"x-ratelimit-remaining-{kind}", str(int(rl_remaining[t]))),
+                (f"x-ratelimit-reset-{kind}", go_duration(window_end(now_unix, names[e]) - now_unix))]
+    return out
+
+
 def request_error_reply(reason: int, detail: int, cur_usage: int, limit_max: int, now_unix: int, tables, qos: int,
                         token: bytes, model: str):
     """-> (status, header, header value, message)"""
@@ -106,10 +141,8 @@ def request_error_reply(reason: int, detail: int, cur_usage: int, limit_max: int
         value, msg = "include_usage for stream_options not set", "no stream with usage option available"
     elif reason == abi.R_RATE_LIMIT:
         rule = tables.qos_rule_names[qos][detail]
-        w = WINDOW[rule]
-        end = now_unix - ((now_unix + 62135596800) % w) + w
         msg = '{"ruleName":"%s","overLimit":true,"currentUsage":%d,"limitMax":%d,"expiresAt":"%s"}' % (
-            rule, cur_usage, limit_max, _rfc3339(end))
+            rule, cur_usage, limit_max, _rfc3339(window_end(now_unix, rule)))
     elif reason == abi.R_QUOTA:
         ns = tables.token_namespace[int(tables.qos_token[qos])]
         msg = ('{"Identifier":[{"Key":"namespace","Value":%s},{"Key":"quotaname","Value":%s},{"Key":"type","Value":"%s"}],'

@@ -2,6 +2,9 @@
 // (no CUDA headers or runtime needed here: the C ABI is the only thing this file knows about the device).
 #include "arks_host.h"
 
+// weak: the host links against any provider of the C ABI, and one without the report (a CPU stand-in) leaves it null
+extern "C" int arks_set_ratelimit_report(arks_ctx* ctx, int on) __attribute__((weak));
+
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -65,6 +68,8 @@ struct Block {
   int32_t *rqos = nullptr, *rtoken = nullptr, *rpick = nullptr;
   int64_t *cur_usage = nullptr, *limit_max = nullptr, *usage = nullptr;
   uint32_t *model_off = nullptr, *model_len = nullptr, *bpe = nullptr;
+  uint8_t* rl_entry = nullptr;  // 2 per row: the rate-limit report (arks_set_ratelimit_report)
+  int64_t *rl_limit = nullptr, *rl_remaining = nullptr;
   // bookkeeping
   uint32_t n = 0;
   size_t bytes = 0, tok_bytes = 0;
@@ -145,6 +150,7 @@ struct Batcher::Impl {
   std::mutex cfg_mu;  // config calls among themselves
   NameBook names;     // generation -> names (published under cfg_mu, read by any stream thread)
   std::atomic<bool> precharge{false};  // N4: response batches carry the streams' estimates
+  std::atomic<bool> rl_report{false};  // request decisions carry the rate-limit report
   int swap_in(arks_prepared* p);
   int publish(arks_prepared* p, const NameTables* nm);
   std::condition_variable cv_work, cv_space, cv_done;
@@ -180,6 +186,7 @@ struct Batcher::Impl {
       b.rqos = new int32_t[m]; b.rtoken = new int32_t[m]; b.rpick = new int32_t[m];
       b.cur_usage = new int64_t[m]; b.limit_max = new int64_t[m];
       b.model_off = new uint32_t[m]; b.model_len = new uint32_t[m]; b.bpe = new uint32_t[m];
+      b.rl_entry = new uint8_t[2 * (size_t)m]; b.rl_limit = new int64_t[2 * (size_t)m]; b.rl_remaining = new int64_t[2 * (size_t)m];
     } else {
       b.qos = pinned<int32_t>(m);
       b.gen = pinned<uint32_t>(m);
@@ -471,19 +478,28 @@ struct Batcher::Impl {
       const uint32_t lo = f.req.lo, hi = f.req.hi;
       int rc = f.rc_req;
       if (rc == 0) {
+        // a batch run without the rate-limit report leaves these arrays as they are: no figures
+        memset(b.rl_entry + 2 * (size_t)lo, ARKS_RL_NONE, 2 * (size_t)(hi - lo));
         arks_request_result rr{b.reason + lo, b.detail + lo, b.rflags + lo, b.rqos + lo, b.rtoken + lo, b.rpick + lo, b.cur_usage + lo,
-                               b.limit_max + lo, b.model_off + lo, b.model_len + lo, b.bpe + lo};
+                               b.limit_max + lo, b.model_off + lo, b.model_len + lo, b.bpe + lo, b.rl_entry + 2 * (size_t)lo,
+                               b.rl_limit + 2 * (size_t)lo, b.rl_remaining + 2 * (size_t)lo};
         rc = arks_wait_request(ctx, f.slot, &rr);
       }
       lap(t_device);
       for (uint32_t i = lo; i < hi; i++) {
         RequestDecision d{};
+        d.rl_entry[0] = d.rl_entry[1] = ARKS_RL_NONE;
         if (rc) d.reason = kReasonHostError;
         else {
           d.reason = b.reason[i]; d.detail = b.detail[i]; d.flags = b.rflags[i];
           d.qos = b.rqos[i]; d.token = b.rtoken[i]; d.pick = b.rpick[i];
           d.cur_usage = b.cur_usage[i]; d.limit_max = b.limit_max[i];
           d.model_off = b.model_off[i]; d.model_len = b.model_len[i]; d.bpe_count = b.bpe[i];
+          for (int t = 0; t < 2; t++) {
+            d.rl_entry[t] = b.rl_entry[2 * (size_t)i + t];
+            d.rl_limit[t] = b.rl_limit[2 * (size_t)i + t];
+            d.rl_remaining[t] = b.rl_remaining[2 * (size_t)i + t];
+          }
         }
         d.cycle = f.cycle; d.index = i - lo; d.now_unix = f.now; d.gen = f.gen;
         b.rcb[i](b.user[i], d);
@@ -666,6 +682,13 @@ int Batcher::SetPrecharge(bool on) {
   return rc;
 }
 bool Batcher::Precharge() const { return p_->precharge.load(std::memory_order_relaxed); }
+int Batcher::SetRatelimitReport(bool on) {
+  if (!arks_set_ratelimit_report) return ARKS_E_NOT_LOADED;  // a provider of the C ABI without the report
+  const int rc = arks_set_ratelimit_report(p_->ctx, on ? 1 : 0);
+  if (!rc) p_->rl_report.store(on, std::memory_order_relaxed);
+  return rc;
+}
+bool Batcher::RatelimitReport() const { return p_->rl_report.load(std::memory_order_relaxed); }
 // config calls are serialised among themselves; the swap itself happens between two cycles
 int Batcher::LoadTables(const arks_tables* t, const NameTables* names) {
   Impl& I = *p_;
@@ -842,6 +865,37 @@ static std::string rfc3339(int64_t unix_s) {
   return b;
 }
 static int64_t window_len(const std::string& rule) { return rule == "rpm" || rule == "tpm" ? 60 : 86400; }  // rate_limiter.go:31-68
+// Go truncates time relative to year 1 (62135596800 s before the epoch)
+int64_t WindowEnd(int64_t now_unix, const std::string& rule) {
+  const int64_t w = window_len(rule);
+  int64_t r = (now_unix + 62135596800LL) % w;
+  if (r < 0) r += w;
+  return now_unix - r + w;
+}
+std::string GoDuration(int64_t seconds) {
+  const int64_t h = seconds / 3600, m = seconds / 60 % 60, s = seconds % 60;
+  if (h) return std::to_string(h) + "h" + std::to_string(m) + "m" + std::to_string(s) + "s";
+  if (m) return std::to_string(m) + "m" + std::to_string(s) + "s";
+  return std::to_string(s) + "s";
+}
+std::vector<Header> RatelimitHeaders(const RequestDecision& d, const NameTables& names) {
+  std::vector<Header> out;
+  if (d.reason != ARKS_R_OK && d.reason != ARKS_R_RATE_LIMIT && d.reason != ARKS_R_QUOTA) return out;
+  if (d.qos < 0 || (size_t)d.qos >= names.qos_rule_names.size()) return out;
+  const std::vector<std::string>& rules = names.qos_rule_names[(size_t)d.qos];
+  if (d.rl_entry[0] == ARKS_RL_NONE && d.rl_entry[1] == ARKS_RL_NONE) return out;
+  if (d.reason == ARKS_R_RATE_LIMIT && d.detail < rules.size())
+    out.push_back({"retry-after", std::to_string(WindowEnd(d.now_unix, rules[d.detail]) - d.now_unix)});
+  static const char* kind[2] = {"requests", "tokens"};
+  for (int t = 0; t < 2; t++) {
+    if (d.rl_entry[t] == ARKS_RL_NONE || d.rl_entry[t] >= rules.size()) continue;
+    const std::string k = kind[t];
+    out.push_back({"x-ratelimit-limit-" + k, std::to_string(d.rl_limit[t])});
+    out.push_back({"x-ratelimit-remaining-" + k, std::to_string(d.rl_remaining[t])});
+    out.push_back({"x-ratelimit-reset-" + k, GoDuration(WindowEnd(d.now_unix, rules[d.rl_entry[t]]) - d.now_unix)});
+  }
+  return out;
+}
 
 ErrorReply RequestErrorReply(const RequestDecision& d, const NameTables& names, std::string_view token, std::string_view body) {
   ErrorReply e{ReasonHttpStatus(d.reason), ReasonHeader(d.reason), "true", ""};
@@ -879,11 +933,8 @@ ErrorReply RequestErrorReply(const RequestDecision& d, const NameTables& names, 
         rule = names.qos_rule_names[(size_t)d.qos][d.detail];
       // expiresAt = now + TTL(key) in the reference (redis_impl.go:104-110; wall clock with nanoseconds, TTL with jitter):
       // the one field that is not a function of the request stream. Here: the end of the rule's fixed window.
-      const int64_t w = window_len(rule);
-      int64_t r = (d.now_unix + 62135596800LL) % w;
-      if (r < 0) r += w;
       e.message = "{\"ruleName\":\"" + rule + "\",\"overLimit\":true,\"currentUsage\":" + std::to_string(d.cur_usage) +
-                  ",\"limitMax\":" + std::to_string(d.limit_max) + ",\"expiresAt\":\"" + rfc3339(d.now_unix - r + w) + "\"}";
+                  ",\"limitMax\":" + std::to_string(d.limit_max) + ",\"expiresAt\":\"" + rfc3339(WindowEnd(d.now_unix, rule)) + "\"}";
       break;
     }
     case ARKS_R_QUOTA: {  // check.go:95-104: QuotaResult.JSON(), quota/types.go:41-55 (Identifier has no json tag)
@@ -1025,7 +1076,13 @@ Action StreamProcessor::OnRequestHeaders(const std::vector<Header>& headers) {
 Action StreamProcessor::OnRequestBody(std::string_view body, uint64_t pick_rand) {
   req_ = b_->HandleRequestBody(token_, body, pick_rand);
   const std::shared_ptr<const NameTables> nm = NamesOf(req_.gen);  // the generation this decision's indices belong to
-  if (req_.reason != ARKS_R_OK) return reply_action(RequestErrorReply(req_, *nm, token_, body));
+  rl_ = RatelimitHeaders(req_, *nm);
+  if (req_.reason != ARKS_R_OK) {
+    Action a = reply_action(RequestErrorReply(req_, *nm, token_, body));
+    a.set_headers.insert(a.set_headers.end(), rl_.begin(), rl_.end());  // behind x-error-* and Content-Type
+    rl_.clear();
+    return a;
+  }
   qos_ = req_.qos;
   gen_ = req_.gen;
   stream_ = req_.flags & 1;
@@ -1053,6 +1110,20 @@ Action StreamProcessor::OnResponseHeaders(const std::vector<Header>& headers) {
   a.clear_route_cache = true;
   // gateway.go:115-121 -> responseErrorProcessing (:281-294): the headers of the reply built so far, an empty message
   if (status_ == 500) return ErrorResponse(500, a.set_headers, "");
+  if (!rl_.empty()) {  // the gateway's rate-limit headers replace the upstream's of the same name
+    auto ours = [&](const Header& h) {
+      std::string k = h.key;
+      for (char& c : k) c = (c >= 'A' && c <= 'Z') ? (char)(c + 32) : c;
+      for (const Header& r : rl_)
+        if (r.key == k) return true;
+      return false;
+    };
+    std::vector<Header> keep;
+    for (const Header& h : a.set_headers)
+      if (!ours(h)) keep.push_back(h);
+    keep.insert(keep.end(), rl_.begin(), rl_.end());
+    a.set_headers = std::move(keep);
+  }
   return a;
 }
 Action StreamProcessor::OnResponseBody(std::string_view body, bool end_of_stream) {
@@ -1163,6 +1234,14 @@ int arks_host_apply_config_named(arks_host_batcher* h, const char* names, uint32
   return h->b->ApplyConfig(&nm);
 }
 int arks_host_set_precharge(arks_host_batcher* h, int on) { return h->b->SetPrecharge(on != 0); }
+int arks_host_set_ratelimit_report(arks_host_batcher* h, int on) { return h->b->SetRatelimitReport(on != 0); }
+int arks_host_ratelimit_headers(arks_host_batcher* h, const RequestDecision* d, char* out, uint32_t out_cap) {
+  std::string o;
+  for (const Header& x : RatelimitHeaders(*d, *h->b->Names().Of(d->gen))) o += x.key + ": " + x.value + "\n";
+  if (o.size() + 1 > out_cap) return -1;
+  memcpy(out, o.c_str(), o.size() + 1);
+  return (int)o.size();
+}
 int arks_host_response_pre(arks_host_batcher* h, int32_t qos, uint32_t gen, uint32_t precharged, const uint8_t* body, uint32_t body_len,
                            uint8_t flags, arks_host::ResponseDecision* out) {
   *out = h->b->HandleResponseBody(qos, gen == 0xffffffffu ? h->b->Generation() : gen, std::string_view((const char*)body, body_len), flags, precharged);

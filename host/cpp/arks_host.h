@@ -40,6 +40,10 @@ struct RequestDecision {
   uint32_t gen;      // table generation qos / token refer to: hand it back with the stream's response chunks
   uint32_t model_off, model_len;  // raw span of the body's model string (bit 31 of model_len: contains escapes)
   uint32_t bpe_count;             // BPE tokens of the prompt (0 without a vocabulary)
+  // rate-limit report (Batcher::SetRatelimitReport): [0] the requests figure, [1] the tokens figure; rl_entry is the index in
+  // qos.RateLimits, ARKS_RL_NONE when there is no such figure (and for every row while the report is off)
+  uint8_t rl_entry[2];
+  int64_t rl_limit[2], rl_remaining[2];
 };
 struct ResponseDecision {
   uint8_t reason, counted;
@@ -122,6 +126,10 @@ class Batcher {
   // response batches carry each stream's estimate back so that the accounting adds total_tokens - estimate
   int SetPrecharge(bool on);
   bool Precharge() const;
+  // opt-in (arks_set_ratelimit_report): request decisions carry the rate-limit figures the StreamProcessor turns into the
+  // x-ratelimit-* / retry-after headers. Batches already queued keep the setting they were queued with
+  int SetRatelimitReport(bool on);
+  bool RatelimitReport() const;
 
   // Config change while streams are in flight (qosconfig informer event): the next generation is built and uploaded on
   // the CALLING (config) thread with batches still running (arks_prepare_tables), then swapped in between two cycles
@@ -191,6 +199,7 @@ class StreamProcessor {
   // what the request phase charged for this stream (N4), handed back with every response chunk: the library subtracts it
   // from the one chunk that carries the usage
   uint32_t Estimate() const { return b_->Precharge() && req_.bpe_count != 0xFFFFFFFFu ? req_.bpe_count : 0u; }
+  std::vector<Header> rl_;  // the admitted request's rate-limit headers, for the response headers
 };
 
 // generateErrorResponse, util.go:40-77: status + headers + Content-Type + {"error":{"message":..,"code":..}}
@@ -206,6 +215,12 @@ struct ErrorReply {
 ErrorReply RequestErrorReply(const RequestDecision& d, const NameTables& names, std::string_view token, std::string_view body);
 ErrorReply ResponseErrorReply(const ResponseDecision& d, const NameTables& names, int32_t qos, std::string_view last_chunk);
 std::string DecodeJsonString(std::string_view raw);  // the model name out of its raw span (jsoniter ReadString semantics)
+// end of the fixed window of `rule` ("rpm", ...) that holds now_unix: the 429 body's expiresAt, x-ratelimit-reset-*, retry-after
+int64_t WindowEnd(int64_t now_unix, const std::string& rule);
+std::string GoDuration(int64_t seconds);  // time.Duration.String() of whole seconds: "1s", "1m0s", "23h59m59s"
+// the rate-limit report of a request decision as headers, in wire order: retry-after (a rate-limit 429 only), then limit /
+// remaining / reset of the requests figure, then of the tokens figure; none when the decision carries no figure
+std::vector<Header> RatelimitHeaders(const RequestDecision& d, const NameTables& names);
 
 }  // namespace arks_host
 
@@ -229,6 +244,10 @@ void arks_host_open_loop_lateness(int64_t out[3]);
 void arks_host_open_loop_call_latency(int64_t* buf); /* n entries filled by the next open-loop run: decision - time of the call */
 int arks_host_apply_config(arks_host_batcher* b);
 int arks_host_set_precharge(arks_host_batcher* b, int on);
+int arks_host_set_ratelimit_report(arks_host_batcher* b, int on);
+/* RatelimitHeaders of a decision under the CURRENT names (arks_host_set_names) as "key: value\n" lines; returns the length, -1
+ * if out_cap is too small */
+int arks_host_ratelimit_headers(arks_host_batcher* b, const arks_host::RequestDecision* d, char* out, uint32_t out_cap);
 int arks_host_response_pre(arks_host_batcher* b, int32_t qos, uint32_t gen, uint32_t precharged, const uint8_t* body, uint32_t body_len,
                            uint8_t flags, arks_host::ResponseDecision* out); /* publishes arks_upsert_* / arks_delete_* done on the context */
 // names of the CURRENT generation for the reply shapes of arks_host_stream_transcript / arks_host_*_error_reply (format:

@@ -183,7 +183,13 @@ typedef struct arks_request_result {
   uint32_t* bpe_count;  /* n: BPE tokens of the prompt text (see arks_load_bpe); 0 when no vocabulary is loaded. A side
                          *    output: the reference counts no tokens at request time (check.go:124-126), so this never
                          *    feeds admit/deny unless arks_set_precharge is switched on                              */
+  /* 2n each, filled only for batches run with arks_set_ratelimit_report on: [2i] the requests figure, [2i + 1] the tokens
+   * figure of row i (see there). May be NULL (not copied out) */
+  uint8_t* rl_entry;     /* index in qos.RateLimits of the reported entry; ARKS_RL_NONE: no figure of that kind */
+  int64_t* rl_limit;     /* that entry's limit                                                                   */
+  int64_t* rl_remaining; /* what is left of it                                                                   */
 } arks_request_result;
+#define ARKS_RL_NONE 0xFFu
 #define ARKS_FLAG_METERED 2u /* admitted under arks_set_stream_metering: the host sets ARKS_RESP_METERED on every chunk */
 
 /* ---- response phase (ProcessingRequest_ResponseBody with :status 200, handle_response.go:80-268) ---- */
@@ -349,6 +355,20 @@ int arks_set_precharge(arks_ctx* ctx, int on);
  * definitions, chat-template tokens. Needs a vocabulary: ARKS_E_NOT_LOADED without one, and arks_load_bpe(NULL) is refused
  * while metering is on. Off by default: decisions are the reference's. */
 int arks_set_stream_metering(arks_ctx* ctx, int on);
+/* OPT-IN rate-limit report: what a tenant has left, for the x-ratelimit-* / retry-after headers OpenAI-style clients pace
+ * themselves by. Decisions and counters are the same with it on or off; on, request batches fill
+ * arks_request_result.rl_entry / rl_limit / rl_remaining (the result block grows by 34 bytes a row). Read when a batch is run,
+ * so an asynchronous submit keeps the setting it was queued with. For a row that reached the limiter (reason ARKS_R_OK,
+ * ARKS_R_RATE_LIMIT or ARKS_R_QUOTA), with rows applied in index order and `a` = the admitted rows of its qos entry in the
+ * batch up to and including it (every admitted one for a denied row):
+ *   request-type entry j (rpm / rpd): remaining = max(0, limit_j - (counter + a x entries of that rule)), the counter as of
+ *                                     the batch's start: the count right after this row's decision;
+ *   token-type entry j (tpm / tpd):   remaining = max(0, limit_j - counter), the value the admission check read (the batch's
+ *                                     start; a pre-charge of the same batch, arks_set_precharge, is not subtracted).
+ * The requests figure is the request-type entry with the least remaining (the first in qos.RateLimits order on a tie), the
+ * tokens figure likewise among token-type entries; ARKS_RL_NONE when the qos entry has no rule of that kind, and for both
+ * figures of every other row (not resolved, refused before the limiter, ARKS_R_QUOTA_CONFIG). Off by default. */
+int arks_set_ratelimit_report(arks_ctx* ctx, int on);
 
 /* routing churn (BASELINE config 5): replace the weights of one endpoint's backends in place */
 int arks_update_endpoint_weights(arks_ctx* ctx, uint32_t endpoint, uint32_t n, const int32_t* weights);
