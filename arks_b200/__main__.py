@@ -52,6 +52,9 @@ def parse_args(argv=None):
     p.add_argument("--gateway.ratelimit-headers", dest="ratelimit_headers", action="store_true",
                    help="send x-ratelimit-{limit,remaining,reset}-{requests,tokens} on every decided request and retry-after on "
                         "rate-limit 429s (off by default: the reference sends none)")
+    p.add_argument("--ratelimiter.sliding-window", dest="sliding_window", action="store_true",
+                   help="admit against the current window plus the previous window's remaining share, so that no burst across "
+                        "a window boundary exceeds a limit (off by default: the reference's fixed window)")
     return p.parse_args(argv)
 
 
@@ -64,6 +67,16 @@ def configure_ratelimit_headers(engine, batcher, args):
     if batcher is not None:
         batcher.b.set_ratelimit_report(True)
     engine.set_ratelimit_report(True)
+
+
+def configure_sliding_window(engine, batcher, args):
+    """--ratelimiter.sliding-window as library calls (arks_set_sliding_window), through the compiled batcher when there is one
+    (its stream state machine shapes the reset / retry headers). Without the flag: no call at all."""
+    if not args.sliding_window:
+        return
+    if batcher is not None:
+        batcher.b.set_sliding_window(True)
+    engine.set_sliding_window(True)
 
 
 def configure_bpe(engine, args, load=None):
@@ -234,6 +247,7 @@ def main(argv=None) -> int:
         batcher = extproc.CompiledBatcher(cpphost.Batcher(cpphost.load(cpphost.build()), g._h, max_batch=args.max_batch,
                                                           max_bytes=args.max_bytes))
     configure_ratelimit_headers(g, batcher, args)  # before Assembly.start() publishes the first generation
+    configure_sliding_window(g, batcher, args)
     status_out = None if args.status_out == "-" else open(args.status_out, "a")
     asm = Assembly(g, args, batcher=batcher, status_out=status_out).start()
     print(f"arks_b200 gateway: gRPC :{asm.grpc_port}, http :{asm.http_port}, metrics :{asm.metrics_port}, device {args.device}, "

@@ -82,7 +82,7 @@ class ArksRequestBatch(C.Structure):
 class ArksRequestResult(C.Structure):
     _fields_ = [("reason", u8p), ("detail", u8p), ("flags", u8p), ("qos", i32p), ("token", i32p), ("pick", i32p),
                 ("cur_usage", i64p), ("limit_max", i64p), ("model_off", u32p), ("model_len", u32p), ("bpe_count", u32p),
-                ("rl_entry", u8p), ("rl_limit", i64p), ("rl_remaining", i64p)]
+                ("rl_entry", u8p), ("rl_limit", i64p), ("rl_remaining", i64p), ("rl_reset", u32p), ("rl_retry", u32p)]
 
 
 RL_NONE = 0xFF  # ARKS_RL_NONE: no rate-limit figure of that kind (arks_set_ratelimit_report)
@@ -179,9 +179,12 @@ class RequestResult:
     rl_entry: np.ndarray = None
     rl_limit: np.ndarray = None
     rl_remaining: np.ndarray = None
+    # sliding window with the report (arks_set_sliding_window): rl_reset [n, 2] like the figures, rl_retry [n]
+    rl_reset: np.ndarray = None
+    rl_retry: np.ndarray = None
 
     @classmethod
-    def empty(cls, n, report: bool = False):
+    def empty(cls, n, report: bool = False, sliding: bool = False):
         r = cls(np.full(n, 255, np.uint8), np.zeros(n, np.uint8), np.zeros(n, np.uint8), np.full(n, -9, np.int32),
                 np.full(n, -9, np.int32), np.full(n, -9, np.int32), np.zeros(n, np.int64), np.zeros(n, np.int64),
                 np.full(n, 0xEEEEEEEE, np.uint32), np.full(n, 0xEEEEEEEE, np.uint32), np.full(n, 0xEEEEEEEE, np.uint32))
@@ -189,6 +192,9 @@ class RequestResult:
             r.rl_entry = np.full((n, 2), 0xEE, np.uint8)
             r.rl_limit = np.full((n, 2), -9, np.int64)
             r.rl_remaining = np.full((n, 2), -9, np.int64)
+            if sliding:
+                r.rl_reset = np.full((n, 2), 0xEEEEEEEE, np.uint32)
+                r.rl_retry = np.full(n, 0xEEEEEEEE, np.uint32)
         return r
 
     def c_struct(self) -> ArksRequestResult:
@@ -196,13 +202,17 @@ class RequestResult:
                                  ptr(self.qos, i32p), ptr(self.token, i32p), ptr(self.pick, i32p),
                                  ptr(self.cur_usage, i64p), ptr(self.limit_max, i64p), ptr(self.model_off, u32p),
                                  ptr(self.model_len, u32p), ptr(self.bpe_count, u32p), ptr(self.rl_entry, u8p),
-                                 ptr(self.rl_limit, i64p), ptr(self.rl_remaining, i64p))
+                                 ptr(self.rl_limit, i64p), ptr(self.rl_remaining, i64p), ptr(self.rl_reset, u32p),
+                                 ptr(self.rl_retry, u32p))
 
     def report(self):
         """the rate-limit report columns, or {} when the result was not asked for them"""
         if self.rl_entry is None:
             return {}
-        return {"rl_entry": self.rl_entry, "rl_limit": self.rl_limit, "rl_remaining": self.rl_remaining}
+        out = {"rl_entry": self.rl_entry, "rl_limit": self.rl_limit, "rl_remaining": self.rl_remaining}
+        if self.rl_reset is not None:
+            out.update(rl_reset=self.rl_reset, rl_retry=self.rl_retry)
+        return out
 
     def fields(self):
         """the arrays the reference's decision determines (bpe_count has its own oracle: tests/test_bpe.py)"""

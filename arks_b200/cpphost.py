@@ -22,7 +22,9 @@ class RequestDecision(C.Structure):
                 ("index", C.c_uint32), ("now_unix", C.c_int64), ("gen", C.c_uint32), ("model_off", C.c_uint32),
                 ("model_len", C.c_uint32), ("bpe_count", C.c_uint32),
                 # rate-limit report: [0] requests, [1] tokens (rl_entry 0xFF: no such figure)
-                ("rl_entry", C.c_uint8 * 2), ("rl_limit", C.c_int64 * 2), ("rl_remaining", C.c_int64 * 2)]
+                ("rl_entry", C.c_uint8 * 2), ("rl_limit", C.c_int64 * 2), ("rl_remaining", C.c_int64 * 2),
+                # sliding window with the report: rl_sliding 1, the projected reset [requests, tokens] and retry seconds
+                ("rl_reset", C.c_uint32 * 2), ("rl_retry", C.c_uint32), ("rl_sliding", C.c_uint8)]
 
 
 class ResponseDecision(C.Structure):
@@ -41,7 +43,7 @@ REQ_DTYPE = np.dtype(RequestDecision)
 RESP_DTYPE = np.dtype(ResponseDecision)
 EXPORTED = ["arks_host_create", "arks_host_destroy", "arks_host_set_fixed_clock", "arks_host_request", "arks_host_response",
             "arks_host_stats", "arks_host_run_requests", "arks_host_run_responses", "arks_host_open_loop_requests",
-            "arks_host_stream_transcript", "arks_host_load_tables", "arks_host_apply_config", "arks_host_set_precharge", "arks_host_set_ratelimit_report", "arks_host_ratelimit_headers", "arks_host_response_pre", "arks_host_set_names", "arks_host_request_error_reply",
+            "arks_host_stream_transcript", "arks_host_load_tables", "arks_host_apply_config", "arks_host_set_precharge", "arks_host_set_ratelimit_report", "arks_host_set_sliding_window", "arks_host_ratelimit_headers", "arks_host_response_pre", "arks_host_set_names", "arks_host_request_error_reply",
             "arks_host_response_error_reply", "arks_host_load_tables_named", "arks_host_apply_config_named",
             "arks_host_response_error_reply_gen"]
 
@@ -76,6 +78,7 @@ def load(path: str = LIB):
     L.arks_host_apply_config_named.argtypes = [vp, C.c_char_p, C.c_uint32]
     L.arks_host_set_precharge.argtypes = [vp, C.c_int]
     L.arks_host_set_ratelimit_report.argtypes = [vp, C.c_int]
+    L.arks_host_set_sliding_window.argtypes = [vp, C.c_int]
     L.arks_host_ratelimit_headers.argtypes = [vp, C.POINTER(RequestDecision), C.c_char_p, C.c_uint32]
     L.arks_host_response_pre.argtypes = [vp, C.c_int32, C.c_uint32, C.c_uint32, C.c_char_p, C.c_uint32, C.c_uint8, C.POINTER(ResponseDecision)]
     L.arks_host_reset_tail.argtypes = [vp]
@@ -148,6 +151,11 @@ class Batcher:
         """request decisions carry the rate-limit figures and the stream state machine sends x-ratelimit-* / retry-after"""
         if self.L.arks_host_set_ratelimit_report(self._h, int(bool(on))):
             raise RuntimeError("arks_host_set_ratelimit_report failed")
+
+    def set_sliding_window(self, on: bool):
+        """the limiter's sliding window (arks_set_sliding_window); with the report on, decisions carry reset / retry times"""
+        if self.L.arks_host_set_sliding_window(self._h, int(bool(on))):
+            raise RuntimeError("arks_host_set_sliding_window failed")
 
     def ratelimit_headers(self, d: RequestDecision):
         """[(key, value)] the stream state machine adds for decision `d` (names of its generation)"""

@@ -8,6 +8,7 @@
 //   state (replaces Redis, pkg/gateway/ratelimiter/redis_impl.go + pkg/gateway/quota/redis_impl.go):
 //     rate[rule][qos]   int64   counter of the CURRENT fixed window of `rule` (cache_key.go:73-80); the host
 //                               zeroes rate[rule][*] when floor(now/W) advances, which is what a new Redis key is
+//     rate[4+rule][qos] int64   the window before it (0 when time skipped it), read by the sliding window only
 //     quota[quota][3]   int64   cumulative usage, never reset (quota/redis_impl.go:38-48)
 //   per batch: bodies (16-byte aligned spans), tokens, a batch-local group table (qos -> arrivals), results.
 //
@@ -90,7 +91,7 @@ struct DevTables {
   const uint32_t* ep_backend_off;
   const int32_t* backend_weight;
   // state
-  long long* rate;   // [4][n_qos]
+  long long* rate;   // [8][n_qos]: planes 0..3 the current window of each rule, 4..7 the previous one
   long long* quota;  // [n_quotas][3]
   long long* qdelta; // [n_quotas][3] increments not yet folded into the other GPUs' copies, or null (single-owner keys)
   long long* metrics; // [n_qos][ARKS_METRIC_COLS] Prometheus series (include/arks_gateway.h), or null when not enabled
@@ -145,7 +146,14 @@ struct ReqDev {  // request batch, device resident
   // null when the report is off
   uint8_t* rl_entry;
   long long* rl_limit;
-  long long* rl_remaining;  // last: the scan kernels' parameter offsets stay as they were
+  long long* rl_remaining;
+  // sliding window (arks_set_sliding_window): the limiter reads cur + floor(prev * win_left / W) per rule, win_left = W - (now
+  // - window start) in 1..W. With the report also on, rl_reset (2n) and rl_retry (n) take the projected seconds, else null
+  int sliding;
+  uint32_t prev_ok;  // bit r: rate plane 4 + r is the previous window of rule r; a clear bit reads as 0 (time skipped it)
+  uint32_t win_left[4];
+  uint32_t* rl_reset;
+  uint32_t* rl_retry;  // last: the scan kernels' parameter offsets stay as they were
 };
 
 struct RespDev {
@@ -1150,7 +1158,36 @@ __global__ void __launch_bounds__(kWdWarps * 32) warp_request_kernel(DevTables T
 //     k = min over request-type entries j of  max(0, floor((limit_j - cur_rule(j) - 1) / cnt_rule(j)) + 1)
 // are admitted (k = 0 if any token-type entry or quota item is already over) and every later one is denied by
 // the first entry that is over with `k` admissions applied.
+// With the sliding window (arks_set_sliding_window) cur_rule is the estimate cur + floor(prev * (W - e) / W) throughout: the
+// share is one number per rule for the whole batch, so the closed form holds as it is. Increments still go to cur.
 // ------------------------------------------------------------------------------------------------
+// floor(p * m / w) exactly for 0 < m <= w <= 86 400 and any int64 p, without a 128-bit product: p = q*w + r, 0 <= r < w, so
+// the result is q*m + floor(r*m / w); |q*m| <= |p| + w and r*m < w*w both fit
+__device__ __forceinline__ long long share_of(long long p, long long m, long long w) {
+  long long q = p / w, r = p % w;
+  if (r < 0) { r += w; q -= 1; }
+  return q * m + r * m / w;
+}
+// The estimate d seconds from now with no further traffic, C (current window) and P (previous window) clamped at 0, left = W - e:
+// C + floor(P (left - d) / W) while the current window lasts, floor(C (left + W - d) / W) through the next one, 0 after that.
+// Non-increasing in d, so the first d it satisfies a bound is found by bisection over [0, left + W]
+__device__ __forceinline__ unsigned long long projected(long long c, long long p, long long d, long long left, long long w) {
+  if (d < left) return (unsigned long long)c + (unsigned long long)share_of(p, left - d, w);
+  if (d < left + w) return (unsigned long long)share_of(c, left + w - d, w);
+  return 0ull;
+}
+// the first d with projected(d) <= bound (bound >= 0); projected(left + W) = 0 always qualifies
+__device__ unsigned long long first_at_most(long long c, long long p, long long left, long long w, unsigned long long bound) {
+  c = c < 0 ? 0 : c;
+  p = p < 0 ? 0 : p;
+  long long lo = 0, hi = left + w;
+  while (lo < hi) {
+    const long long mid = (lo + hi) >> 1;
+    if (projected(c, p, mid, left, w) <= bound) hi = mid;
+    else lo = mid + 1;
+  }
+  return (unsigned long long)lo;
+}
 // kernel 2b: one block per hot group sweeps the slot column once, front to back, and hands every member its arrival
 // rank (members with a smaller request index). n / 256 coalesced tile loads per hot group.
 __global__ void __launch_bounds__(256) rank_hot_groups_kernel(ReqDev B) {
@@ -1210,6 +1247,7 @@ __global__ void __launch_bounds__(128) limit_admit_kernel(DevTables T, ReqDev B)
   // ---- phase A (per lane): how many arrivals of my group can be admitted
   uint32_t rl0 = 0, rl1 = 0;
   long long n_g = 0, k = 0, cur[4] = {0, 0, 0, 0}, cnt[4] = {0, 0, 0, 0}, q_cur = 0, q_lim = 0;
+  long long sh[4] = {0, 0, 0, 0};  // sliding window: the previous window's share, already added to cur
   int32_t qt = ARKS_QUOTA_NONE;
   int quota_fail = -1;  // first over-limit item
   // Everything a decision may need is fetched in three rounds of independent loads (the kernel is a chain of dependent
@@ -1230,6 +1268,16 @@ __global__ void __launch_bounds__(128) limit_admit_kernel(DevTables T, ReqDev B)
     i0 = T.quota_item_off[qs]; i1 = T.quota_item_off[qs + 1];
     b0 = T.ep_backend_off[es]; b1 = T.ep_backend_off[es + 1];
     const long long qu0 = T.quota[(size_t)qs * 3], qu1 = T.quota[(size_t)qs * 3 + 1], qu2 = T.quota[(size_t)qs * 3 + 2];
+    if (B.sliding) {  // prev lives in planes 4..7 and changes only between batches (roll_windows, the generation carry)
+      long long pv[4];
+#pragma unroll
+      for (int r = 0; r < 4; r++) pv[r] = (B.prev_ok >> r & 1) ? T.rate[(size_t)(4 + r) * T.n_qos + qos] : 0;
+#pragma unroll
+      for (int r = 0; r < 4; r++) {
+        sh[r] = share_of(pv[r], B.win_left[r], (r & 1) ? 86400 : 60);
+        cur[r] = (long long)((unsigned long long)cur[r] + (unsigned long long)sh[r]);
+      }
+    }
     for (uint32_t j = rl0; j < rl1; j++) cnt[T.rl_rule[j]]++;
     k = n_g;
     for (uint32_t j = rl0; j < rl1; j++) {
@@ -1264,6 +1312,7 @@ __global__ void __launch_bounds__(128) limit_admit_kernel(DevTables T, ReqDev B)
   // ---- phase C: decision, commit, pick
   uint8_t rq_e = 0xFF, tk_e = 0xFF;  // rate-limit report: the requests figure and the tokens figure (scalars: no local memory)
   long long rq_lim = 0, rq_rem = 0, tk_lim = 0, tk_rem = 0;
+  uint32_t rq_reset = 0, tk_reset = 0, retry = 0;
   if (slot >= 0) {
     const bool admitted = k >= n_g ? true : k <= 0 ? false : rank < k;
     if (!admitted) {
@@ -1298,6 +1347,26 @@ __global__ void __launch_bounds__(128) limit_admit_kernel(DevTables T, ReqDev B)
         if (rule < 2 && (rq_e == 0xFF || rem < rq_rem)) { rq_e = (uint8_t)(j - rl0); rq_lim = lim; rq_rem = rem; }
         if (rule >= 2 && (tk_e == 0xFF || rem < tk_rem)) { tk_e = (uint8_t)(j - rl0); tk_lim = lim; tk_rem = rem; }
       }
+      // sliding window: when each figure's estimate reaches 0 and, for a rate-limit 429, when the denying entry admits again
+      // (never: the time it reaches 0). C is the counter as the figure reads it without the share, P the previous window
+      if (B.rl_reset) {
+#pragma unroll
+        for (int t = 0; t < 2; t++) {
+          const uint8_t e = t ? tk_e : rq_e;
+          if (e == 0xFF) continue;
+          const int rule = T.rl_rule[rl0 + e];
+          const long long c = (rule < 2 ? cur[rule] + a * cnt[rule] : cur[rule]) - sh[rule];
+          const long long w = (rule & 1) ? 86400 : 60;
+          const long long p = (B.prev_ok >> rule & 1) ? T.rate[(size_t)(4 + rule) * T.n_qos + qos] : 0;
+          (t ? tk_reset : rq_reset) = (uint32_t)first_at_most(c, p, B.win_left[rule], w, 0ull);
+        }
+        if (reason == ARKS_R_RATE_LIMIT) {
+          const int rule = T.rl_rule[rl0 + detail];
+          const long long w = (rule & 1) ? 86400 : 60, req = rule < 2 ? 1 : 0;
+          const long long c = cur_out - sh[rule], p = (B.prev_ok >> rule & 1) ? T.rate[(size_t)(4 + rule) * T.n_qos + qos] : 0;
+          retry = (uint32_t)first_at_most(c, p, B.win_left[rule], w, lim_out >= req ? (unsigned long long)(lim_out - req) : 0ull);
+        }
+      }
     }
     // N4 (opt-in): the estimate is charged when the micro-batch commits; nobody reads T.rate here. Metered rows (N5) are
     // charged by meter_charge_kernel instead
@@ -1322,8 +1391,8 @@ __global__ void __launch_bounds__(128) limit_admit_kernel(DevTables T, ReqDev B)
     if (B.st_flags[i] & 0x80) {
       long long adm = k < n_g ? (k < 0 ? 0 : k) : n_g;
       if (adm > 0) {
-        if (cnt[0]) T.rate[(size_t)0 * T.n_qos + qos] = cur[0] + adm * cnt[0];
-        if (cnt[1]) T.rate[(size_t)1 * T.n_qos + qos] = cur[1] + adm * cnt[1];
+        if (cnt[0]) T.rate[(size_t)0 * T.n_qos + qos] = cur[0] - sh[0] + adm * cnt[0];
+        if (cnt[1]) T.rate[(size_t)1 * T.n_qos + qos] = cur[1] - sh[1] + adm * cnt[1];
       }
     }
   }
@@ -1340,6 +1409,10 @@ __global__ void __launch_bounds__(128) limit_admit_kernel(DevTables T, ReqDev B)
     reinterpret_cast<uchar2*>(B.rl_entry)[i] = make_uchar2(rq_e, tk_e);
     reinterpret_cast<longlong2*>(B.rl_limit)[i] = make_longlong2(rq_lim, tk_lim);
     reinterpret_cast<longlong2*>(B.rl_remaining)[i] = make_longlong2(rq_rem, tk_rem);
+  }
+  if (B.rl_reset) {
+    reinterpret_cast<uint2*>(B.rl_reset)[i] = make_uint2(rq_reset, tk_reset);
+    B.rl_retry[i] = retry;
   }
 }
 
@@ -1952,6 +2025,8 @@ struct arks_ctx {
   bool precharge = false;              // N4 (arks_set_precharge)
   bool meter = false;                  // N5 (arks_set_stream_metering)
   bool rl_report = false;              // arks_set_ratelimit_report
+  bool sliding = false;                // arks_set_sliding_window
+  uint32_t prev_ok = 0xF;              // bit r: plane 4 + r holds the window before last_win[r] (else it reads as 0)
   bool split = false;                  // fast path: two lanes per document in pass A (fast_*_kernel2), ARKS_SPLIT=1; measured slower
   bool walk8 = true;                   // fast path, pass B: the step inlined eight times (true) or one copy in a loop
   int regroup = 1;                     // fast path: regroup a block's documents by structure between passes A and B
@@ -2008,6 +2083,7 @@ struct arks_ctx {
     cudaEvent_t req_ran = nullptr, resp_ran = nullptr;  // the slot's device buffers are free again (kernels done)
     uint32_t req_fetch_n = 0, resp_fetch_n = 0;
     bool req_report = false;  // the request batch in this slot was run with the rate-limit report (its result block is longer)
+    bool req_sliding = false; // ... and with the sliding window: the block also holds rl_reset / rl_retry when both are on
     ReqDev rq{};
     RespDev rp{};
     uint32_t req_n = 0, resp_n = 0;
@@ -2191,7 +2267,8 @@ int arks_create(int device, uint32_t max_batch, uint64_t max_batch_bytes, arks_c
 
   CK(cudaMalloc(&ctx->d_lenhist, (size_t)4 * kLenBuckets));
   ctx->result_cap = align_up(n, 256) * 3 + align_up(n * 4, 256) * 6 + align_up(n * 8, 256) * 3 +
-                    align_up(n * 2, 256) + align_up(n * 16, 256) * 2;  // + the rate-limit report's three arrays
+                    align_up(n * 2, 256) + align_up(n * 16, 256) * 2 +  // + the rate-limit report's three arrays
+                    align_up(n * 8, 256) + align_up(n * 4, 256);        // + the sliding window's reset and retry
   CK(cudaMalloc(&ctx->d_result, ctx->result_cap));
   CK(cudaMemset(ctx->d_result, 0, ctx->result_cap));  // the packed block has alignment gaps that the D2H copies too
   return 0;
@@ -2704,7 +2781,7 @@ int arks_prepare_tables(arks_ctx* ctx, const arks_tables* t, arks_prepared** out
   int32_t *n_qos_from = nullptr, *n_quota_from = nullptr;
   {
     int rc;
-    if ((rc = put(nullptr, 0, (void**)&n_rate, (size_t)32 * t->n_qos))) return rc;
+    if ((rc = put(nullptr, 0, (void**)&n_rate, (size_t)64 * t->n_qos))) return rc;  // [8][n_qos]: current and previous windows
     if ((rc = put(nullptr, 0, (void**)&n_quota, (size_t)24 * t->n_quotas))) return rc;
     if ((rc = put(nullptr, 0, (void**)&n_metrics, (size_t)8 * ARKS_METRIC_COLS * t->n_qos))) return rc;
     if ((rc = put(qos_from.data(), (size_t)4 * (t->n_qos + 1), (void**)&n_qos_from))) return rc;
@@ -2775,7 +2852,7 @@ int arks_commit_tables(arks_ctx* ctx, arks_prepared* p) {
       carry_rows_kernel<<<(total + 255) / 256, 256, 0, ctx->stream>>>(dst, src, map, n_new, cols, ds, ss, cm);
       ctx->launches += 1;
     };
-    carry(p->rate, ctx->d_rate, p->d_qos_from, p->n_qos, 4, p->n_qos, ctx->ht.n_qos, 1);
+    carry(p->rate, ctx->d_rate, p->d_qos_from, p->n_qos, 8, p->n_qos, ctx->ht.n_qos, 1);  // both windows, by key
     carry(p->metrics, ctx->d_metrics, p->d_qos_from, p->n_qos, ARKS_METRIC_COLS, 0, 0, 0);
     carry(p->quota, ctx->d_quota, p->d_quota_from, p->n_quotas, 3, 0, 0, 0);
     carry(p->qdelta, ctx->d_qdelta, p->d_quota_from, p->n_quotas, 3, 0, 0, 0);
@@ -2913,6 +2990,11 @@ int arks_set_ratelimit_report(arks_ctx* ctx, int on) {
   ctx->rl_report = on != 0;
   return 0;
 }
+int arks_set_sliding_window(arks_ctx* ctx, int on) {
+  if (!ctx) return ARKS_E_INVALID_ARG;
+  ctx->sliding = on != 0;
+  return 0;
+}
 int arks_set_stream_metering(arks_ctx* ctx, int on) {
   if (!ctx) return ARKS_E_INVALID_ARG;
   if (on && !ctx->bpe_on) return fail(ctx, ARKS_E_NOT_LOADED, "stream metering needs a vocabulary (arks_load_bpe)");
@@ -2935,19 +3017,37 @@ int arks_update_endpoint_weights(arks_ctx* ctx, uint32_t ep, uint32_t n, const i
   return 0;
 }
 
-// fixed-window roll-over: a new window is a new Redis key, i.e. every counter of that rule reads 0
+// fixed-window roll-over: a new window is a new Redis key, i.e. every counter of that rule reads 0. The window that ends
+// becomes the previous one (plane 4 + rule) when the new one follows it directly; when time skipped a window the previous
+// plane is marked stale instead (prev_ok: reads as 0) rather than cleared. Kept whether or not the sliding window is on, so
+// that switching it on at any batch is exact. Rules that roll together are handled as one span of planes: one copy (a
+// skipped rule's plane inside it is copied too and marked stale) and one memset, so a roll-over of every rule queues two
+// operations, no kernel
 static int roll_windows(arks_ctx* ctx, int64_t now) {
   for (int r = 0; r < 4; r++)
     if (window_start(now, r) < ctx->last_win[r])
       return fail(ctx, ARKS_E_TIME_WENT_BACK, "now_unix %lld is before the current %s window", (long long)now,
                   r == 0 ? "rpm" : r == 1 ? "rpd" : r == 2 ? "tpm" : "tpd");
+  bool rolled[4] = {false, false, false, false}, adjacent[4] = {false, false, false, false};
   for (int r = 0; r < 4; r++) {
-    int64_t ws = window_start(now, r);
+    const int64_t ws = window_start(now, r);
     if (ws != ctx->last_win[r]) {
-      if (ctx->last_win[r] != INT64_MIN && ctx->ht.n_qos)
-        CK(cudaMemsetAsync(ctx->d_rate + (size_t)r * ctx->ht.n_qos, 0, (size_t)8 * ctx->ht.n_qos, ctx->stream));
+      rolled[r] = ctx->last_win[r] != INT64_MIN;  // the first window of all starts from the zeroed planes
+      adjacent[r] = ws - kRuleWindow[r] == ctx->last_win[r];
       ctx->last_win[r] = ws;
     }
+  }
+  const size_t nq = ctx->ht.n_qos;
+  for (int a = 0; a < 4;) {
+    if (!rolled[a]) { a++; continue; }
+    int b = a;
+    bool copy = false;
+    for (; b < 4 && rolled[b]; b++) copy |= adjacent[b];
+    if (nq && copy) CK(cudaMemcpyAsync(ctx->d_rate + (size_t)(4 + a) * nq, ctx->d_rate + (size_t)a * nq, 8 * nq * (b - a),
+                                       cudaMemcpyDeviceToDevice, ctx->stream));
+    if (nq) CK(cudaMemsetAsync(ctx->d_rate + (size_t)a * nq, 0, 8 * nq * (b - a), ctx->stream));
+    for (int r = a; r < b; r++) ctx->prev_ok = adjacent[r] ? ctx->prev_ok | 1u << r : ctx->prev_ok & ~(1u << r);
+    a = b;
   }
   return 0;
 }
@@ -3077,22 +3177,25 @@ int arks_stage_request_batch(arks_ctx* ctx, const arks_request_batch* b) {
   return 0;
 }
 
-// offsets of the 11 result arrays inside the packed result block of a batch of n (dense: one D2H for any n), and with the
-// rate-limit report 3 more behind them (rl_entry 2n bytes, rl_limit and rl_remaining 2n int64). Returns the block's size
-constexpr int kReqResultArrays = 11, kReqReportArrays = 3;
-static size_t result_offsets(size_t n, bool report, size_t offs[kReqResultArrays + kReqReportArrays + 1]) {
+// offsets of the 11 result arrays inside the packed result block of a batch of n (dense: one D2H for any n), with the
+// rate-limit report 3 more behind them (rl_entry 2n bytes, rl_limit and rl_remaining 2n int64), and with the sliding window
+// too 2 more (rl_reset 2n, rl_retry n uint32). Returns the block's size
+constexpr int kReqResultArrays = 11, kReqReportArrays = 5;
+static size_t result_offsets(size_t n, bool report, bool sliding, size_t offs[kReqResultArrays + kReqReportArrays + 1]) {
   const size_t a1 = align_up(n, 16), a4 = align_up(n * 4, 16), a8 = align_up(n * 8, 16);
   offs[0] = 0; offs[1] = a1; offs[2] = 2 * a1; offs[3] = 3 * a1; offs[4] = offs[3] + a4; offs[5] = offs[4] + a4;
   offs[6] = offs[5] + a4; offs[7] = offs[6] + a8; offs[8] = offs[7] + a8;
   offs[9] = offs[8] + a4; offs[10] = offs[9] + a4; offs[11] = offs[10] + a4;
   if (!report) return offs[kReqResultArrays];
   offs[12] = offs[11] + align_up(n * 2, 16); offs[13] = offs[12] + align_up(n * 16, 16); offs[14] = offs[13] + align_up(n * 16, 16);
-  return offs[kReqResultArrays + kReqReportArrays];
+  if (!sliding) return offs[14];
+  offs[15] = offs[14] + align_up(n * 8, 16); offs[16] = offs[15] + align_up(n * 4, 16);
+  return offs[16];
 }
 // Micro-batches write their result rows straight into the slot's pinned host block (zero copy over PCIe: the block is
 // device-addressable under unified addressing): no D2H copy node between the last kernel and the host's wake-up.
 constexpr uint32_t kZeroCopyRows = 2048;
-static void carve_request(arks_ctx* ctx, ReqDev& r, size_t batch_n, bool report, uint8_t* result_base) {
+static void carve_request(arks_ctx* ctx, ReqDev& r, size_t batch_n, bool report, bool sliding, uint8_t* result_base) {
   const size_t n = ctx->max_batch;
   uint8_t* p = ctx->d_inter;
   r.st_reason = p; p += align_up(n, 256);
@@ -3109,7 +3212,7 @@ static void carve_request(arks_ctx* ctx, ReqDev& r, size_t batch_n, bool report,
   r.hot_list = (int32_t*)p; p += align_up((n / kHotGroup + 2) * 4, 256);
   r.hotrank = (int32_t*)p;
   size_t offs[kReqResultArrays + kReqReportArrays + 1];
-  result_offsets(batch_n, report, offs);
+  result_offsets(batch_n, report, sliding, offs);
   uint8_t* q = result_base;
   r.reason = q + offs[0];
   r.detail = q + offs[1];
@@ -3125,6 +3228,8 @@ static void carve_request(arks_ctx* ctx, ReqDev& r, size_t batch_n, bool report,
   r.rl_entry = report ? q + offs[11] : nullptr;
   r.rl_limit = report ? (long long*)(q + offs[12]) : nullptr;
   r.rl_remaining = report ? (long long*)(q + offs[13]) : nullptr;
+  r.rl_reset = report && sliding ? (uint32_t*)(q + offs[14]) : nullptr;
+  r.rl_retry = report && sliding ? (uint32_t*)(q + offs[15]) : nullptr;
 }
 
 // A warp is as slow as its slowest body and pays for every code path any of its lanes takes, so a small batch is spread
@@ -3172,8 +3277,12 @@ int arks_run_request_batch(arks_ctx* ctx, int64_t now_unix) {
   ReqDev& r = sl.rq;
   sl.req_zc = n <= kZeroCopyRows && sl.h_req_result;
   sl.req_report = ctx->rl_report;
-  carve_request(ctx, r, n, sl.req_report, sl.req_zc ? sl.h_req_result : ctx->d_result);
+  sl.req_sliding = ctx->sliding;
+  carve_request(ctx, r, n, sl.req_report, sl.req_sliding, sl.req_zc ? sl.h_req_result : ctx->d_result);
   r.meter = ctx->meter ? 1 : 0;
+  r.sliding = sl.req_sliding ? 1 : 0;
+  r.prev_ok = ctx->prev_ok;
+  for (int k = 0; k < 4; k++) r.win_left[k] = (uint32_t)(window_start(now_unix, k) + kRuleWindow[k] - now_unix);
   // batch-local group table sized to the batch (2x, power of two); the three arrays are contiguous
   uint32_t g = 64;
   while (g < 2 * n) g <<= 1;
@@ -3263,7 +3372,7 @@ static int enqueue_request_fetch(arks_ctx* ctx) {
   sl.req_fetch_n = (uint32_t)n;
   if (n == 0) return 0;
   size_t offs[kReqResultArrays + kReqReportArrays + 1];
-  const size_t bytes = result_offsets(n, sl.req_report, offs);
+  const size_t bytes = result_offsets(n, sl.req_report, sl.req_sliding, offs);
   if (!sl.req_zc) CK(cudaMemcpyAsync(sl.h_req_result, ctx->d_result, bytes, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaEventRecord(sl.req_done, ctx->stream));
   return 0;
@@ -3287,7 +3396,7 @@ static int finish_request_fetch(arks_ctx* ctx, int slot, arks_request_result* ou
   CK(wait_event_polling(sl.req_done));
   const uint8_t* h = sl.h_req_result;
   size_t offs[kReqResultArrays + kReqReportArrays + 1];
-  result_offsets(n, sl.req_report, offs);
+  result_offsets(n, sl.req_report, sl.req_sliding, offs);
   memcpy(out->reason, h + offs[0], n);
   memcpy(out->detail, h + offs[1], n);
   memcpy(out->flags, h + offs[2], n);
@@ -3303,6 +3412,10 @@ static int finish_request_fetch(arks_ctx* ctx, int slot, arks_request_result* ou
     if (out->rl_entry) memcpy(out->rl_entry, h + offs[11], n * 2);
     if (out->rl_limit) memcpy(out->rl_limit, h + offs[12], n * 16);
     if (out->rl_remaining) memcpy(out->rl_remaining, h + offs[13], n * 16);
+  }
+  if (sl.req_report && sl.req_sliding) {  // the sliding window's reset / retry: only with both switches on
+    if (out->rl_reset) memcpy(out->rl_reset, h + offs[14], n * 8);
+    if (out->rl_retry) memcpy(out->rl_retry, h + offs[15], n * 4);
   }
   return 0;
 }
@@ -3643,6 +3756,23 @@ int arks_snapshot_rate(arks_ctx* ctx, int64_t now_unix, int64_t* counters) {
   for (size_t q = 0; q < nq; q++)
     for (int r = 0; r < 4; r++)
       counters[q * 4 + r] = window_start(now_unix, r) == ctx->last_win[r] ? tmp[(size_t)r * nq + q] : 0;
+  return 0;
+}
+int arks_snapshot_rate_prev(arks_ctx* ctx, int64_t now_unix, int64_t* counters) {
+  if (!ctx || !ctx->loaded) return ARKS_E_NOT_LOADED;
+  CK(cudaSetDevice(ctx->device));
+  CK(cudaStreamSynchronize(ctx->stream));
+  const size_t nq = ctx->ht.n_qos;
+  std::vector<long long> tmp(8 * nq + 1);
+  if (nq) CK(cudaMemcpy(tmp.data(), ctx->d_rate, 64 * nq, cudaMemcpyDeviceToHost));
+  // the window before now's: plane 4 + r while now is in the last window run (unless time skipped it), plane r itself when
+  // now is in the next one
+  for (size_t q = 0; q < nq; q++)
+    for (int r = 0; r < 4; r++) {
+      const int64_t ws = window_start(now_unix, r);
+      counters[q * 4 + r] = ws == ctx->last_win[r] ? ((ctx->prev_ok >> r & 1) ? tmp[(size_t)(4 + r) * nq + q] : 0)
+                            : ws - kRuleWindow[r] == ctx->last_win[r] ? tmp[(size_t)r * nq + q] : 0;
+    }
   return 0;
 }
 

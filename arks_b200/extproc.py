@@ -342,7 +342,7 @@ class Batcher:
                 RequestBatch.from_lists([i["body"] for i in reqs], [i["token"] for i in reqs], now, pick_rand=rnd))
             for k, i in enumerate(reqs):
                 i["out"] = {f: v[k] for f, v in r.fields().items()}
-                i["out"].update({f: tuple(v[k]) for f, v in r.report().items()})  # with the rate-limit report on
+                i["out"].update({f: tuple(v[k]) if v.ndim > 1 else int(v[k]) for f, v in r.report().items()})  # report on
                 i["out"].update(now=now, gen=gen)
                 i["ev"].set()
         if resps:
@@ -384,7 +384,7 @@ class CompiledBatcher:
         return {"reason": d.reason, "detail": d.detail, "flags": d.flags, "qos": d.qos, "token": d.token, "pick": d.pick,
                 "cur_usage": d.cur_usage, "limit_max": d.limit_max, "now": d.now_unix, "gen": d.gen,
                 "model_off": d.model_off, "model_len": d.model_len, "rl_entry": tuple(d.rl_entry), "rl_limit": tuple(d.rl_limit),
-                "rl_remaining": tuple(d.rl_remaining)}
+                "rl_remaining": tuple(d.rl_remaining), **({"rl_reset": tuple(d.rl_reset), "rl_retry": d.rl_retry} if d.rl_sliding else {})}
 
     def response(self, body: bytes, qos: int, flags: int, gen: int = None):
         d = self.b.response(qos, body, flags, gen)
@@ -499,13 +499,14 @@ class ExtProcServer:
         out = self.batcher.request(body, token)
         reason = int(out["reason"])
         rl = replies.ratelimit_headers(reason, int(out["detail"]), int(out["qos"]), int(out.get("now", 0)), out.get("rl_entry"),
-                                       out.get("rl_limit"), out.get("rl_remaining"), self.names_of(out.get("gen")))
+                                       out.get("rl_limit"), out.get("rl_remaining"), self.names_of(out.get("gen")),
+                                       out.get("rl_reset"), out.get("rl_retry"))
         if reason != abi.R_OK:
             ml = int(out.get("model_len", 0))
             raw = body[int(out.get("model_off", 0)):int(out.get("model_off", 0)) + (ml & 0x7FFFFFFF)]
             st, h, v, m = replies.request_error_reply(reason, int(out["detail"]), int(out["cur_usage"]), int(out["limit_max"]),
                                                       int(out.get("now", 0)), self.names_of(out.get("gen")), int(out["qos"]), token,
-                                                      replies.decode_model(raw, bool(ml >> 31)))
+                                                      replies.decode_model(raw, bool(ml >> 31)), out.get("rl_retry"))
             r = error_response(st, h, v, m)
             r.immediate_response.headers.MergeFrom(_set_headers(rl))  # behind x-error-* and Content-Type
             return r, (-1, None), False, []

@@ -68,6 +68,7 @@ def lib():
         L.arks_set_precharge.argtypes = [vp, C.c_int]
         L.arks_set_stream_metering.argtypes = [vp, C.c_int]
         L.arks_set_ratelimit_report.argtypes = [vp, C.c_int]
+        L.arks_set_sliding_window.argtypes = [vp, C.c_int]
         L.arks_table_generation.restype = C.c_uint32
         L.arks_table_generation.argtypes = [vp]
         L.arks_update_endpoint_weights.argtypes = [vp, C.c_uint32, C.c_uint32, abi.i32p]
@@ -98,6 +99,7 @@ def lib():
         L.arks_set_quota_usage.argtypes = [vp, C.c_uint32, abi.i64p]
         L.arks_incr_quota_usage.argtypes = [vp, C.c_uint32, abi.i64p]
         L.arks_snapshot_rate.argtypes = [vp, C.c_int64, abi.i64p]
+        L.arks_snapshot_rate_prev.argtypes = [vp, C.c_int64, abi.i64p]
         L.arks_sync_quota_usage.argtypes = [vp, C.c_int, abi.u32p, abi.i64p, abi.u8p]
         L.arks_enable_metrics.argtypes = [vp, C.c_int]
         L.arks_snapshot_metrics.argtypes = [vp, abi.i64p]
@@ -119,7 +121,7 @@ def lib():
 
 EXPORTED = [  # every symbol include/arks_gateway.h declares (checked by tests/test_abi.py)
     "arks_abi_version", "arks_create", "arks_destroy", "arks_last_error", "arks_load_tables", "arks_table_generation", "arks_load_bpe", "arks_set_precharge",
-    "arks_set_stream_metering", "arks_set_ratelimit_report", "arks_load_bpe_vocab", "arks_bind_model_vocab",
+    "arks_set_stream_metering", "arks_set_ratelimit_report", "arks_set_sliding_window", "arks_load_bpe_vocab", "arks_bind_model_vocab",
     "arks_prepare_tables", "arks_commit_tables", "arks_discard_prepared", "arks_upsert_token", "arks_delete_token", "arks_upsert_quota",
     "arks_delete_quota", "arks_upsert_endpoint", "arks_delete_endpoint", "arks_config_prepare", "arks_find_quota", "arks_find_qos",
     "arks_update_endpoint_weights", "arks_extract_bearer", "arks_submit_request_batch",
@@ -127,7 +129,7 @@ EXPORTED = [  # every symbol include/arks_gateway.h declares (checked by tests/t
     "arks_fetch_request_result", "arks_stage_response_batch", "arks_run_response_batch",
     "arks_fetch_response_result", "arks_submit_request_async", "arks_wait_request", "arks_submit_response_async",
     "arks_wait_response", "arks_select_slot", "arks_set_profiling", "arks_last_kernel_ms", "arks_stream", "arks_launch_count", "arks_last_declined", "arks_last_staging_route", "arks_enable_metrics", "arks_snapshot_metrics", "arks_sync_quota_usage", "arks_alloc_pinned", "arks_free_pinned", "arks_snapshot_quota",
-    "arks_set_quota_usage", "arks_incr_quota_usage", "arks_snapshot_rate", "arks_take_quota_delta",
+    "arks_set_quota_usage", "arks_incr_quota_usage", "arks_snapshot_rate", "arks_snapshot_rate_prev", "arks_take_quota_delta",
     "arks_apply_quota_delta", "arks_quota_delta_dev", "arks_fold_quota_delta_dev", "arks_enable_quota_sharing",
     "arks_comm_unique_id", "arks_comm_init", "arks_comm_set_shared", "arks_fold_quota_allreduce", "arks_comm_destroy",
     "arks_export_quota_delta_dev",
@@ -151,6 +153,7 @@ class Gateway:
             raise ArksError(rc, msg)
         self.tables = None
         self.ratelimit_report = False
+        self.sliding_window = False
 
     def close(self):
         if getattr(self, "_h", None):
@@ -276,6 +279,13 @@ class Gateway:
         self._ck(lib().arks_set_ratelimit_report(self._h, int(bool(on))))
         self.ratelimit_report = bool(on)
 
+    def set_sliding_window(self, on: bool):
+        """opt-in: the limiter reads cur + floor(prev * (W - e) / W) per rule instead of the fixed window's cur (see
+        include/arks_gateway.h arks_set_sliding_window); with the rate-limit report on, results also carry rl_reset [n, 2] and
+        rl_retry [n]"""
+        self._ck(lib().arks_set_sliding_window(self._h, int(bool(on))))
+        self.sliding_window = bool(on)
+
     @property
     def generation(self) -> int:
         """table generation the qos / token indices of request results refer to (carry it with the stream)"""
@@ -287,7 +297,7 @@ class Gateway:
 
     # ---- HandleRequestBody for a micro-batch of streams
     def handle_request_body(self, b: RequestBatch, out: RequestResult | None = None) -> RequestResult:
-        r = out if out is not None else RequestResult.empty(b.n, self.ratelimit_report)
+        r = out if out is not None else RequestResult.empty(b.n, self.ratelimit_report, self.sliding_window)
         bs, rs = b.c_struct(), r.c_struct()
         self._ck(lib().arks_submit_request_batch(self._h, C.byref(bs), C.byref(rs)))
         return r
@@ -327,7 +337,7 @@ class Gateway:
         self._ck(lib().arks_run_request_batch(self._h, int(now_unix)))
 
     def fetch_request(self, n: int, out: RequestResult | None = None) -> RequestResult:
-        r = out if out is not None else RequestResult.empty(n, self.ratelimit_report)
+        r = out if out is not None else RequestResult.empty(n, self.ratelimit_report, self.sliding_window)
         rs = r.c_struct()
         self._ck(lib().arks_fetch_request_result(self._h, C.byref(rs)))
         return r
@@ -409,6 +419,12 @@ class Gateway:
     def snapshot_rate(self, now_unix: int) -> np.ndarray:
         out = np.zeros((self.tables.n_qos, 4), np.int64)
         self._ck(lib().arks_snapshot_rate(self._h, int(now_unix), abi.ptr(out, abi.i64p)))
+        return out
+
+    def snapshot_rate_prev(self, now_unix: int) -> np.ndarray:
+        """the counters of the windows just before now_unix's (the sliding window's prev; 0 when not adjacent)"""
+        out = np.zeros((self.tables.n_qos, 4), np.int64)
+        self._ck(lib().arks_snapshot_rate_prev(self._h, int(now_unix), abi.ptr(out, abi.i64p)))
         return out
 
     def set_quota_usage(self, quota: int, usage):

@@ -101,28 +101,32 @@ def go_duration(seconds: int) -> str:
 RATELIMIT_HEADERS = tuple(f"x-ratelimit-{w}-{k}" for k in ("requests", "tokens") for w in ("limit", "remaining", "reset"))
 
 
-def ratelimit_headers(reason: int, detail: int, qos: int, now_unix: int, rl_entry, rl_limit, rl_remaining, tables):
+def ratelimit_headers(reason: int, detail: int, qos: int, now_unix: int, rl_entry, rl_limit, rl_remaining, tables, rl_reset=None,
+                      rl_retry=None):
     """the headers of the rate-limit report (arks_set_ratelimit_report) for one request decision, in wire order: retry-after
     on a rate-limit 429 (until the denying entry's window ends), then limit / remaining / reset of the requests figure, then
-    of the tokens figure. A figure without an entry (abi.RL_NONE) adds nothing; [] when the decision carries no report."""
+    of the tokens figure. A figure without an entry (abi.RL_NONE) adds nothing; [] when the decision carries no report.
+    Under the sliding window (arks_set_sliding_window) the decision also carries rl_reset / rl_retry, the seconds the device
+    projected, and those replace the window ends."""
     if reason not in (abi.R_OK, abi.R_RATE_LIMIT, abi.R_QUOTA) or rl_entry is None or all(int(e) == abi.RL_NONE for e in rl_entry):
         return []
     names = tables.qos_rule_names[qos]
     out = []
     if reason == abi.R_RATE_LIMIT:
-        out.append(("retry-after", str(window_end(now_unix, names[detail]) - now_unix)))
+        out.append(("retry-after", str(int(rl_retry) if rl_retry is not None else window_end(now_unix, names[detail]) - now_unix)))
     for t, kind in enumerate(("requests", "tokens")):
         e = int(rl_entry[t])
         if e == abi.RL_NONE:
             continue
         out += [(f"x-ratelimit-limit-{kind}", str(int(rl_limit[t]))), (f"x-ratelimit-remaining-{kind}", str(int(rl_remaining[t]))),
-                (f"x-ratelimit-reset-{kind}", go_duration(window_end(now_unix, names[e]) - now_unix))]
+                (f"x-ratelimit-reset-{kind}", go_duration(int(rl_reset[t]) if rl_reset is not None else window_end(now_unix, names[e]) - now_unix))]
     return out
 
 
 def request_error_reply(reason: int, detail: int, cur_usage: int, limit_max: int, now_unix: int, tables, qos: int,
-                        token: bytes, model: str):
-    """-> (status, header, header value, message)"""
+                        token: bytes, model: str, rl_retry=None):
+    """-> (status, header, header value, message). `rl_retry`: the sliding window's retry time of a rate-limit 429
+    (arks_set_sliding_window with the report), which expiresAt then names instead of the window end"""
     status, header = abi.REASON_HTTP.get(reason, (500, "x-error-rate-limit"))
     value, msg = "true", ""
     if reason == abi.R_NO_TOKEN:
@@ -142,7 +146,7 @@ def request_error_reply(reason: int, detail: int, cur_usage: int, limit_max: int
     elif reason == abi.R_RATE_LIMIT:
         rule = tables.qos_rule_names[qos][detail]
         msg = '{"ruleName":"%s","overLimit":true,"currentUsage":%d,"limitMax":%d,"expiresAt":"%s"}' % (
-            rule, cur_usage, limit_max, _rfc3339(window_end(now_unix, rule)))
+            rule, cur_usage, limit_max, _rfc3339(now_unix + int(rl_retry) if rl_retry is not None else window_end(now_unix, rule)))
     elif reason == abi.R_QUOTA:
         ns = tables.token_namespace[int(tables.qos_token[qos])]
         msg = ('{"Identifier":[{"Key":"namespace","Value":%s},{"Key":"quotaname","Value":%s},{"Key":"type","Value":"%s"}],'

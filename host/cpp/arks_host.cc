@@ -4,6 +4,7 @@
 
 // weak: the host links against any provider of the C ABI, and one without the report (a CPU stand-in) leaves it null
 extern "C" int arks_set_ratelimit_report(arks_ctx* ctx, int on) __attribute__((weak));
+extern "C" int arks_set_sliding_window(arks_ctx* ctx, int on) __attribute__((weak));
 
 #include <stdio.h>
 #include <stdlib.h>
@@ -70,6 +71,7 @@ struct Block {
   uint32_t *model_off = nullptr, *model_len = nullptr, *bpe = nullptr;
   uint8_t* rl_entry = nullptr;  // 2 per row: the rate-limit report (arks_set_ratelimit_report)
   int64_t *rl_limit = nullptr, *rl_remaining = nullptr;
+  uint32_t *rl_reset = nullptr, *rl_retry = nullptr;  // 2 and 1 per row: the sliding window's times (arks_set_sliding_window)
   // bookkeeping
   uint32_t n = 0;
   size_t bytes = 0, tok_bytes = 0;
@@ -151,6 +153,7 @@ struct Batcher::Impl {
   NameBook names;     // generation -> names (published under cfg_mu, read by any stream thread)
   std::atomic<bool> precharge{false};  // N4: response batches carry the streams' estimates
   std::atomic<bool> rl_report{false};  // request decisions carry the rate-limit report
+  std::atomic<bool> sliding{false};    // the limiter runs the sliding window
   int swap_in(arks_prepared* p);
   int publish(arks_prepared* p, const NameTables* nm);
   std::condition_variable cv_work, cv_space, cv_done;
@@ -187,6 +190,7 @@ struct Batcher::Impl {
       b.cur_usage = new int64_t[m]; b.limit_max = new int64_t[m];
       b.model_off = new uint32_t[m]; b.model_len = new uint32_t[m]; b.bpe = new uint32_t[m];
       b.rl_entry = new uint8_t[2 * (size_t)m]; b.rl_limit = new int64_t[2 * (size_t)m]; b.rl_remaining = new int64_t[2 * (size_t)m];
+      b.rl_reset = new uint32_t[2 * (size_t)m]; b.rl_retry = new uint32_t[m];
     } else {
       b.qos = pinned<int32_t>(m);
       b.gen = pinned<uint32_t>(m);
@@ -480,9 +484,11 @@ struct Batcher::Impl {
       if (rc == 0) {
         // a batch run without the rate-limit report leaves these arrays as they are: no figures
         memset(b.rl_entry + 2 * (size_t)lo, ARKS_RL_NONE, 2 * (size_t)(hi - lo));
+        memset(b.rl_retry + lo, 0xFF, 4 * (size_t)(hi - lo));  // ... and these without the sliding window (no time is 2^32 - 1 s)
         arks_request_result rr{b.reason + lo, b.detail + lo, b.rflags + lo, b.rqos + lo, b.rtoken + lo, b.rpick + lo, b.cur_usage + lo,
                                b.limit_max + lo, b.model_off + lo, b.model_len + lo, b.bpe + lo, b.rl_entry + 2 * (size_t)lo,
-                               b.rl_limit + 2 * (size_t)lo, b.rl_remaining + 2 * (size_t)lo};
+                               b.rl_limit + 2 * (size_t)lo, b.rl_remaining + 2 * (size_t)lo, b.rl_reset + 2 * (size_t)lo,
+                               b.rl_retry + lo};
         rc = arks_wait_request(ctx, f.slot, &rr);
       }
       lap(t_device);
@@ -499,6 +505,12 @@ struct Batcher::Impl {
             d.rl_entry[t] = b.rl_entry[2 * (size_t)i + t];
             d.rl_limit[t] = b.rl_limit[2 * (size_t)i + t];
             d.rl_remaining[t] = b.rl_remaining[2 * (size_t)i + t];
+          }
+          if (b.rl_retry[i] != 0xFFFFFFFFu) {
+            d.rl_sliding = 1;
+            d.rl_reset[0] = b.rl_reset[2 * (size_t)i];
+            d.rl_reset[1] = b.rl_reset[2 * (size_t)i + 1];
+            d.rl_retry = b.rl_retry[i];
           }
         }
         d.cycle = f.cycle; d.index = i - lo; d.now_unix = f.now; d.gen = f.gen;
@@ -689,6 +701,13 @@ int Batcher::SetRatelimitReport(bool on) {
   return rc;
 }
 bool Batcher::RatelimitReport() const { return p_->rl_report.load(std::memory_order_relaxed); }
+int Batcher::SetSlidingWindow(bool on) {
+  if (!arks_set_sliding_window) return ARKS_E_NOT_LOADED;  // a provider of the C ABI without the sliding window
+  const int rc = arks_set_sliding_window(p_->ctx, on ? 1 : 0);
+  if (!rc) p_->sliding.store(on, std::memory_order_relaxed);
+  return rc;
+}
+bool Batcher::SlidingWindow() const { return p_->sliding.load(std::memory_order_relaxed); }
 // config calls are serialised among themselves; the swap itself happens between two cycles
 int Batcher::LoadTables(const arks_tables* t, const NameTables* names) {
   Impl& I = *p_;
@@ -885,14 +904,15 @@ std::vector<Header> RatelimitHeaders(const RequestDecision& d, const NameTables&
   const std::vector<std::string>& rules = names.qos_rule_names[(size_t)d.qos];
   if (d.rl_entry[0] == ARKS_RL_NONE && d.rl_entry[1] == ARKS_RL_NONE) return out;
   if (d.reason == ARKS_R_RATE_LIMIT && d.detail < rules.size())
-    out.push_back({"retry-after", std::to_string(WindowEnd(d.now_unix, rules[d.detail]) - d.now_unix)});
+    out.push_back({"retry-after", std::to_string(d.rl_sliding ? (int64_t)d.rl_retry : WindowEnd(d.now_unix, rules[d.detail]) - d.now_unix)});
   static const char* kind[2] = {"requests", "tokens"};
   for (int t = 0; t < 2; t++) {
     if (d.rl_entry[t] == ARKS_RL_NONE || d.rl_entry[t] >= rules.size()) continue;
     const std::string k = kind[t];
     out.push_back({"x-ratelimit-limit-" + k, std::to_string(d.rl_limit[t])});
     out.push_back({"x-ratelimit-remaining-" + k, std::to_string(d.rl_remaining[t])});
-    out.push_back({"x-ratelimit-reset-" + k, GoDuration(WindowEnd(d.now_unix, rules[d.rl_entry[t]]) - d.now_unix)});
+    out.push_back({"x-ratelimit-reset-" + k,
+                   GoDuration(d.rl_sliding ? (int64_t)d.rl_reset[t] : WindowEnd(d.now_unix, rules[d.rl_entry[t]]) - d.now_unix)});
   }
   return out;
 }
@@ -934,7 +954,8 @@ ErrorReply RequestErrorReply(const RequestDecision& d, const NameTables& names, 
       // expiresAt = now + TTL(key) in the reference (redis_impl.go:104-110; wall clock with nanoseconds, TTL with jitter):
       // the one field that is not a function of the request stream. Here: the end of the rule's fixed window.
       e.message = "{\"ruleName\":\"" + rule + "\",\"overLimit\":true,\"currentUsage\":" + std::to_string(d.cur_usage) +
-                  ",\"limitMax\":" + std::to_string(d.limit_max) + ",\"expiresAt\":\"" + rfc3339(WindowEnd(d.now_unix, rule)) + "\"}";
+                  ",\"limitMax\":" + std::to_string(d.limit_max) + ",\"expiresAt\":\"" +
+                  rfc3339(d.rl_sliding ? d.now_unix + (int64_t)d.rl_retry : WindowEnd(d.now_unix, rule)) + "\"}";
       break;
     }
     case ARKS_R_QUOTA: {  // check.go:95-104: QuotaResult.JSON(), quota/types.go:41-55 (Identifier has no json tag)
@@ -1235,6 +1256,7 @@ int arks_host_apply_config_named(arks_host_batcher* h, const char* names, uint32
 }
 int arks_host_set_precharge(arks_host_batcher* h, int on) { return h->b->SetPrecharge(on != 0); }
 int arks_host_set_ratelimit_report(arks_host_batcher* h, int on) { return h->b->SetRatelimitReport(on != 0); }
+int arks_host_set_sliding_window(arks_host_batcher* h, int on) { return h->b->SetSlidingWindow(on != 0); }
 int arks_host_ratelimit_headers(arks_host_batcher* h, const RequestDecision* d, char* out, uint32_t out_cap) {
   std::string o;
   for (const Header& x : RatelimitHeaders(*d, *h->b->Names().Of(d->gen))) o += x.key + ": " + x.value + "\n";

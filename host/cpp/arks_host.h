@@ -44,6 +44,10 @@ struct RequestDecision {
   // qos.RateLimits, ARKS_RL_NONE when there is no such figure (and for every row while the report is off)
   uint8_t rl_entry[2];
   int64_t rl_limit[2], rl_remaining[2];
+  // sliding window with the report (Batcher::SetSlidingWindow): rl_sliding 1 when the batch ran with both; then rl_reset[t] is
+  // the seconds until figure t's estimate reaches 0 and rl_retry the seconds until a rate-limit 429's entry admits again
+  uint32_t rl_reset[2], rl_retry;
+  uint8_t rl_sliding;
 };
 struct ResponseDecision {
   uint8_t reason, counted;
@@ -130,6 +134,10 @@ class Batcher {
   // x-ratelimit-* / retry-after headers. Batches already queued keep the setting they were queued with
   int SetRatelimitReport(bool on);
   bool RatelimitReport() const;
+  // opt-in (arks_set_sliding_window): the limiter admits against the current window plus the previous window's remaining
+  // share; with the report on, the reset / retry headers and expiresAt name the projected times. Queued batches keep theirs
+  int SetSlidingWindow(bool on);
+  bool SlidingWindow() const;
 
   // Config change while streams are in flight (qosconfig informer event): the next generation is built and uploaded on
   // the CALLING (config) thread with batches still running (arks_prepare_tables), then swapped in between two cycles
@@ -245,6 +253,7 @@ void arks_host_open_loop_call_latency(int64_t* buf); /* n entries filled by the 
 int arks_host_apply_config(arks_host_batcher* b);
 int arks_host_set_precharge(arks_host_batcher* b, int on);
 int arks_host_set_ratelimit_report(arks_host_batcher* b, int on);
+int arks_host_set_sliding_window(arks_host_batcher* b, int on);
 /* RatelimitHeaders of a decision under the CURRENT names (arks_host_set_names) as "key: value\n" lines; returns the length, -1
  * if out_cap is too small */
 int arks_host_ratelimit_headers(arks_host_batcher* b, const arks_host::RequestDecision* d, char* out, uint32_t out_cap);

@@ -188,6 +188,9 @@ typedef struct arks_request_result {
   uint8_t* rl_entry;     /* index in qos.RateLimits of the reported entry; ARKS_RL_NONE: no figure of that kind */
   int64_t* rl_limit;     /* that entry's limit                                                                   */
   int64_t* rl_remaining; /* what is left of it                                                                   */
+  /* filled only for batches run with both arks_set_ratelimit_report and arks_set_sliding_window on (see there). May be NULL */
+  uint32_t* rl_reset;    /* 2n: seconds until the estimate of that figure's entry reaches 0 with no further traffic      */
+  uint32_t* rl_retry;    /* n: a rate-limit 429 (ARKS_R_RATE_LIMIT): seconds until the denying entry admits again; else 0 */
 } arks_request_result;
 #define ARKS_RL_NONE 0xFFu
 #define ARKS_FLAG_METERED 2u /* admitted under arks_set_stream_metering: the host sets ARKS_RESP_METERED on every chunk */
@@ -369,6 +372,21 @@ int arks_set_stream_metering(arks_ctx* ctx, int on);
  * tokens figure likewise among token-type entries; ARKS_RL_NONE when the qos entry has no rule of that kind, and for both
  * figures of every other row (not resolved, refused before the limiter, ARKS_R_QUOTA_CONFIG). Off by default. */
 int arks_set_ratelimit_report(arks_ctx* ctx, int on);
+/* OPT-IN sliding-window rate limits. The fixed window lets a tenant send its whole limit at the end of one window and again
+ * at the start of the next; the sliding window weighs in the previous window's count by how much of it still overlaps the
+ * last W seconds. Each rule r (W = 60 s for rpm / tpm, 86 400 s for rpd / tpd, e = now - its window start) keeps `cur`
+ * (the current window, as without the switch) and `prev` (the window before it; 0 if it was never written or time skipped
+ * it), and the limiter reads
+ *   est = cur + floor(prev * (W - e) / W)     (exact for any int64 prev; the sum wraps modulo 2^64)
+ * wherever it read cur: admission, the 429's currentUsage, the report's figures. Increments still go to cur; quotas are
+ * not affected. prev is kept whether or not the switch is on, so switching on at any batch is exact. Read when a batch is
+ * run, so an asynchronous submit keeps the setting it was queued with.
+ * With the rate-limit report also on, each figure gets rl_reset: the least d with E(d) = 0, where C (the figure's counter
+ * without the share) and P = prev are clamped at 0 and E(d) = C + floor(P (W - e - d) / W) for d < W - e,
+ * floor(C (2W - e - d) / W) for d < 2W - e, 0 after that; and a rate-limit 429 gets rl_retry: the least d with
+ * E(d) + req <= limit for the denying entry (req 1 for rpm / rpd, 0 for tpm / tpd), rl_reset's d when there is none.
+ * Off by default: the reference's fixed window. */
+int arks_set_sliding_window(arks_ctx* ctx, int on);
 
 /* routing churn (BASELINE config 5): replace the weights of one endpoint's backends in place */
 int arks_update_endpoint_weights(arks_ctx* ctx, uint32_t endpoint, uint32_t n, const int32_t* weights);
@@ -462,6 +480,8 @@ int arks_sync_quota_usage(arks_ctx* ctx, int mode, uint32_t* status_present /* n
 int arks_incr_quota_usage(arks_ctx* ctx, uint32_t quota, const int64_t delta[3]); /* IncrUsage */
 /* rate counters of the CURRENT windows (value 0 if the stored window is older than now_unix's) */
 int arks_snapshot_rate(arks_ctx* ctx, int64_t now_unix, int64_t* counters /* 4 * n_qos */);
+/* rate counters of the windows just before now_unix's (what arks_set_sliding_window calls prev; 0 when not adjacent) */
+int arks_snapshot_rate_prev(arks_ctx* ctx, int64_t now_unix, int64_t* counters /* 4 * n_qos */);
 
 /* multi-GPU: ArksQuotas shared across GPUs (SURVEY §8e). Off by default (tenant-sharded, single-owner keys, exact).
  * When enabled (before arks_load_tables) every response-phase quota increment is also accumulated in a per-GPU delta
