@@ -39,6 +39,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
 #include <deque>
 #include <dlfcn.h>
 #include <nccl.h>  // types only: the entry points are looked up with dlsym at arks_comm_init
@@ -537,6 +538,18 @@ __device__ __forceinline__ void resolve_request(const DevTables& T, const ReqDev
 }
 
 // ------------------------------------------------------------------------------------------------
+// Programmatic dependent launch (DESIGN.md §5). Every kernel of a batch's chain is launched by launch_chained(): the grid
+// may start while the kernel before it drains. pdl_open() at the top of each block lets the next grid be launched as soon
+// as every block of this one has started. pdl_wait() returns once the kernel before has completed and its writes are
+// visible. Before it a kernel reads only the batch's staged inputs and the generation's config tables and writes only
+// registers and shared memory; every global write and every read of state an earlier kernel writes comes after it.
+// Every kernel executes pdl_wait() on every path, early exits included: one that skipped it could complete before its
+// own predecessor, and the kernel behind it would then run ahead of both.
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ void pdl_open() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+
+// ------------------------------------------------------------------------------------------------
 // Lane assignment: bodies are handed to lanes in order of length (counting sort, arbitrary order inside a bucket). Lanes of a warp run in lock step window by window, so a warp is as slow as its longest / densest
 // body; with equal lengths, bodies that share a shape (the completions of one serving stack, the requests of one
 // application) also reach their structure-dense regions in the same windows. Decisions do not depend on the
@@ -548,6 +561,8 @@ __device__ __forceinline__ uint32_t len_bucket(uint32_t len) {
 }
 
 __global__ void len_hist_kernel(const uint32_t* body_len, uint32_t n, uint32_t* hist) {
+  pdl_open();
+  pdl_wait();  // on every path (see pdl_wait)
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   const bool live = i < n;
   const uint32_t b = live ? len_bucket(body_len[i]) : 0xffffffffu;
@@ -558,6 +573,8 @@ static_assert(kLenBuckets == 4096, "len_scan_kernel: one block of 1024 threads, 
 // exclusive scan of the kLenBuckets counters in place (one block of 1024 threads, 4 counters each)
 __global__ void __launch_bounds__(1024) len_scan_kernel(uint32_t* hist) {
   __shared__ uint32_t warp_tot[32];
+  pdl_open();
+  pdl_wait();  // on every path (see pdl_wait)
   const uint32_t t = threadIdx.x;
   uint32_t v[4], sum = 0;
 #pragma unroll
@@ -585,6 +602,8 @@ __global__ void __launch_bounds__(1024) len_scan_kernel(uint32_t* hist) {
   for (int k = 0; k < 4; k++) { hist[4 * t + k] = base; base += v[k]; }
 }
 __global__ void len_scatter_kernel(const uint32_t* body_len, uint32_t n, uint32_t* offs, uint32_t* perm) {
+  pdl_open();
+  pdl_wait();  // on every path (see pdl_wait)
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   const bool live = i < n;
   const uint32_t b = live ? len_bucket(body_len[i]) : 0xffffffffu;
@@ -600,45 +619,56 @@ __global__ void len_scatter_kernel(const uint32_t* body_len, uint32_t n, uint32_
 // ------------------------------------------------------------------------------------------------
 // kernel 1: scan_request — A3 (body parse), A4 (GetQosByToken), A5 (GetModelList) of SURVEY.md §8a
 // ------------------------------------------------------------------------------------------------
-// FROM_LIST: second stage of the two-stage scan — the requests the fast path left to the exact engine (B.slow_list).
+// FROM_LIST: second stage of the two-stage scan — the requests the fast path left to the exact engine (B.slow_list). Its
+// grid is fixed (scan_list_grid) and sized before the list is known: each warp strides over the list's groups of bpw rows.
 template <int SCHED, bool FROM_LIST>
 __global__ void __launch_bounds__(kWarpsPerBlock * 32, kMinBlocks) scan_request_kernel(DevTables T, ReqDev B) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  const uint32_t n = FROM_LIST ? *B.slow_n + 1u : B.n;  // the counter starts at -1 (it is cleared together with the 0xff tables)
-  const uint32_t lane_id = ((blockIdx.x * blockDim.x + threadIdx.x) >> 5) * B.bpw + (threadIdx.x & 31);
-  if (FROM_LIST && ((blockIdx.x * blockDim.x) >> 5) * B.bpw >= n) return;  // nothing left for this block
-  const bool live = (threadIdx.x & 31) < B.bpw && lane_id < n;
-  const uint32_t i = live ? (FROM_LIST ? B.slow_list[lane_id] : B.perm ? B.perm[lane_id] : lane_id) : 0;  // the body this lane parses
-  const uint8_t* body = B.bodies + (live ? B.body_off[i] : 0);
-  const uint32_t len = live ? B.body_len[i] : 0;
-
-  uint32_t stack_words[kStackWords];  // local memory, touched only beyond 32 levels of nesting
   __shared__ __align__(16) JsonSmem<true, false> json_smem;
+  pdl_open();
   const JsonTables tabs = json_smem.stage_async();
-  WindowPipe<kStages> pipe;
-  pipe.start(body, len, smem + (threadIdx.x >> 5) * (kStages * kStageBytes));
+  pdl_wait();  // on every path (see pdl_wait): B.perm, the list and its counter are written by earlier kernels
+  const uint32_t n = FROM_LIST ? *B.slow_n + 1u : B.n;  // the counter starts at -1 (batch_head_kernel clears it)
+  const uint32_t warps = FROM_LIST ? gridDim.x * kWarpsPerBlock : 0u;
+  if (FROM_LIST && ((blockIdx.x * blockDim.x) >> 5) * B.bpw >= n) {  // nothing left for this block
+    cp_async_wait<0>();
+    return;
+  }
+  uint32_t stack_words[kStackWords];  // local memory, touched only beyond 32 levels of nesting
+  for (uint32_t q = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, first = 1;; q += warps, first = 0) {
+    const uint32_t lane_id = q * B.bpw + (threadIdx.x & 31);
+    const bool live = (threadIdx.x & 31) < B.bpw && lane_id < n;
+    const uint32_t i = live ? (FROM_LIST ? B.slow_list[lane_id] : B.perm ? B.perm[lane_id] : lane_id) : 0;  // the body this lane parses
+    const uint8_t* body = B.bodies + (live ? B.body_off[i] : 0);
+    const uint32_t len = live ? B.body_len[i] : 0;
+    WindowPipe<kStages> pipe;
+    pipe.start(body, len, smem + (threadIdx.x >> 5) * (kStages * kStageBytes));
 
-  // GetQosByToken does not need the body, so it runs here, while the automaton tables and the first body windows are
-  // still in flight.
-  int32_t tok = -1;
-  if (live) tok = lookup_token(T, B, i);
-  cp_async_wait<kStages - 1>();  // the table group is the oldest one
-  __syncthreads();
+    // GetQosByToken does not need the body, so it runs here, while the automaton tables and the first body windows are
+    // still in flight.
+    int32_t tok = -1;
+    if (live) tok = lookup_token(T, B, i);
+    if (first) {  // the whole block runs the first round
+      cp_async_wait<kStages - 1>();  // the table group is the oldest one
+      __syncthreads();
+    }
 
-  JsonCold cold;  // rarely touched parse state: local memory on purpose (json_engine.cuh)
-  JsonT m;
-  m.init(K_REQ, body, stack_words, &cold, tabs);
-  feed_pipe<SCHED>(m, pipe, 0);
-  if (!live) return;
-
-  const bool parsed = m.ok_at_end();
-  const uint8_t pstate = !parsed ? PS_BAD
-                                 : (uint8_t)((cold.stream3 == 2 ? PS_STREAM : 0) | (cold.so_present && cold.iu3 == 2 ? PS_STREAM_OK : 0));
-  const uint32_t m_rawlen = parsed ? cold.m_rawlen : 0;
-  B.model_off[i] = m_rawlen ? cold.m_start : 0u;
-  B.model_len[i] = m_rawlen ? (m_rawlen | (cold.m_esc ? 0x80000000u : 0u)) : 0u;
-  B.bpe[i] = 0;
-  resolve_request(T, B, i, body, tok, pstate, cold.m_start, m_rawlen, cold.m_esc);
+    JsonCold cold;  // rarely touched parse state: local memory on purpose (json_engine.cuh)
+    JsonT m;
+    m.init(K_REQ, body, stack_words, &cold, tabs);
+    feed_pipe<SCHED>(m, pipe, 0);
+    if (live) {
+      const bool parsed = m.ok_at_end();
+      const uint8_t pstate = !parsed ? PS_BAD
+                                     : (uint8_t)((cold.stream3 == 2 ? PS_STREAM : 0) | (cold.so_present && cold.iu3 == 2 ? PS_STREAM_OK : 0));
+      const uint32_t m_rawlen = parsed ? cold.m_rawlen : 0;
+      B.model_off[i] = m_rawlen ? cold.m_start : 0u;
+      B.model_len[i] = m_rawlen ? (m_rawlen | (cold.m_esc ? 0x80000000u : 0u)) : 0u;
+      B.bpe[i] = 0;
+      resolve_request(T, B, i, body, tok, pstate, cold.m_start, m_rawlen, cold.m_esc);
+    }
+    if (!FROM_LIST || (q + warps) * B.bpw >= n) break;
+  }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -790,7 +820,9 @@ template <int WALK>
 __global__ void __launch_bounds__(kFastThreads) fast_request_kernel(DevTables T, ReqDev B, int regroup) {
   extern __shared__ __align__(1024) uint8_t smem[];
   FastBlockSmem& sm = *reinterpret_cast<FastBlockSmem*>(smem);
+  pdl_open();
   stage_fast_tables(&sm.tabs, &sm.bar);
+  if (B.perm) pdl_wait();  // the length order is written by the kernels before this one
   const uint32_t base = blockIdx.x * blockDim.x;
   TokProbe probe{};
   {
@@ -803,7 +835,7 @@ __global__ void __launch_bounds__(kFastThreads) fast_request_kernel(DevTables T,
     fast_pass_a(B.bodies + (in ? B.body_off[i] : 0), in && !(regroup & 512) ? B.body_len[i] : 0u, sm);
     sm.slot[threadIdx.x] = a;
   }
-  if (regroup & 256) return;  // timing experiments only (ARKS_REGROUP=257): pass A alone, no results
+  if (regroup & 256) { pdl_wait(); return; }  // timing experiments only (ARKS_REGROUP=257): pass A alone, no results
   regroup &= 255;
   const int notail = regroup & 128;
   regroup &= 127;
@@ -821,6 +853,9 @@ __global__ void __launch_bounds__(kFastThreads) fast_request_kernel(DevTables T,
   const uint32_t len = live ? B.body_len[i] : 0u;
   FastOut o;
   const bool accepted = fast_pass_bc<K_REQ, WALK>(live, body, len, sm, u, o);
+  // The scan above overlaps the kernel before; what follows writes the list, the rows and the group table. On every path
+  // (see pdl_wait)
+  pdl_wait();
   if (!live) return;
   if (!accepted) {
     B.slow_list[atomicAdd(B.slow_n, 1u) + 1u] = i;
@@ -955,7 +990,9 @@ template <int WALK>
 __global__ void __launch_bounds__(kFastThreads, 7) fast_request_kernel2(DevTables T, ReqDev B, int regroup) {
   extern __shared__ __align__(1024) uint8_t smem[];
   FastSplitSmem& sm = *reinterpret_cast<FastSplitSmem*>(smem);
+  pdl_open();
   stage_fast_tables(&sm.tabs, &sm.bar);
+  pdl_wait();  // on every path (see pdl_wait)
   const uint32_t base = blockIdx.x * kSplitDocs, pair = threadIdx.x >> 1;
   const uint32_t own = base + pair;
   const uint32_t len0 = own < B.n ? B.body_len[B.perm ? B.perm[own] : own] : 0u;
@@ -1126,8 +1163,9 @@ __device__ __forceinline__ bool wd_fetch(WdWarpSmem& sm, const uint8_t* src, uin
 __global__ void __launch_bounds__(kWdWarps * 32) warp_request_kernel(DevTables T, ReqDev B) {
   extern __shared__ __align__(1024) uint8_t smem[];
   WdWarpSmem& sm = reinterpret_cast<WdWarpSmem*>(smem)[threadIdx.x >> 5];
+  pdl_open();
   const uint32_t i = blockIdx.x * kWdWarps + (threadIdx.x >> 5);
-  if (i >= B.n) return;
+  if (i >= B.n) { pdl_wait(); return; }  // on every path (see pdl_wait)
   const uint8_t* body = B.bodies + B.body_off[i];
   const uint32_t len = B.body_len[i];
   // GetQosByToken's chain of dependent loads runs in lane 0 while the body is on its way
@@ -1136,6 +1174,7 @@ __global__ void __launch_bounds__(kWdWarps * 32) warp_request_kernel(DevTables T
   if ((threadIdx.x & 31) == 0) tok = lookup_token(T, B, i);
   wd::FastOut o;
   const bool ok = elig && wd_scan_doc<K_REQ>(sm.doc, len, sm, o);
+  pdl_wait();  // the scan above overlaps the kernel before; the list, the rows and the group table come after it
   if ((threadIdx.x & 31) != 0) return;
   if (!ok) {
     B.slow_list[atomicAdd(B.slow_n, 1u) + 1u] = i;
@@ -1192,7 +1231,9 @@ __device__ unsigned long long first_at_most(long long c, long long p, long long 
 // rank (members with a smaller request index). n / 256 coalesced tile loads per hot group.
 __global__ void __launch_bounds__(256) rank_hot_groups_kernel(ReqDev B) {
   __shared__ uint32_t warp_tot[8];
-  const int n_hot = *B.hot_n + 1;  // the counter starts at -1 (it is part of the group-table memset)
+  pdl_open();
+  pdl_wait();  // on every path, the no-hot-group exit included (see pdl_wait)
+  const int n_hot = *B.hot_n + 1;  // the counter starts at -1 (batch_head_kernel clears it with the group table)
   const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   for (int h = blockIdx.x; h < n_hot; h += gridDim.x) {
     const int32_t s = B.hot_list[h];
@@ -1238,6 +1279,8 @@ __global__ void __launch_bounds__(256) rank_hot_groups_kernel(ReqDev B) {
 }
 
 __global__ void __launch_bounds__(128) limit_admit_kernel(DevTables T, ReqDev B) {
+  pdl_open();
+  pdl_wait();  // on every path (see pdl_wait): everything below reads what the scan stage wrote
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   const bool live = i < B.n;
   uint8_t reason = live ? B.st_reason[i] : 0, detail = 0;
@@ -1521,46 +1564,57 @@ __device__ __forceinline__ void account_usage(const DevTables& T, const RespDev&
 }
 
 // complete (non-stream) response bodies: one JSON document per lane.
-// FROM_LIST: second stage of the two-stage scan (the bodies in B.slow_list).
+// FROM_LIST: second stage of the two-stage scan (the bodies in B.slow_list), on a fixed grid (see scan_request_kernel).
 template <int SCHED, bool FROM_LIST>
 __global__ void __launch_bounds__(kWarpsPerBlock * 32, kMinBlocks) scan_response_kernel(DevTables T, RespDev B) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  const uint32_t n = FROM_LIST ? *B.slow_n + 1u : B.n;  // the counter starts at -1 (it is cleared together with the 0xff tables)
-  const uint32_t lane_id = ((blockIdx.x * blockDim.x + threadIdx.x) >> 5) * B.bpw + (threadIdx.x & 31);
-  if (FROM_LIST && ((blockIdx.x * blockDim.x) >> 5) * B.bpw >= n) return;
-  const bool live = (threadIdx.x & 31) < B.bpw && lane_id < n;
-  const uint32_t i = live ? (FROM_LIST ? B.slow_list[lane_id] : B.perm ? B.perm[lane_id] : lane_id) : 0;  // the body this lane parses
-  uint8_t reason = ARKS_R_OK, counted = 0;
-  long long u0 = 0, u1 = 0, u2 = 0;
-  int32_t qos = 0;
-  QosAcct acct;
-  {
-    const uint8_t* body = B.bodies + (live ? B.body_off[i] : 0);
-    const uint8_t fl = live ? B.flags[i] : ARKS_RESP_END_OF_STREAM;
-    const bool pending = !(fl & ARKS_RESP_END_OF_STREAM);  // more of the body is still to come: handle_response.go:141-149
-    qos = live ? B.qos[i] : 0;
-    const uint32_t len = live && !pending && qos >= 0 ? B.body_len[i] : 0;
-    uint32_t stack_words[kStackWords];  // local memory, touched only beyond 32 levels of nesting
-    __shared__ __align__(16) JsonSmem<true, false> json_smem;
-    const JsonTables tabs = json_smem.stage_async();
-    WindowPipe<kStages> pipe;
-    pipe.start(body, len, smem + (threadIdx.x >> 5) * (kStages * kStageBytes));
-    acct = load_qos_acct(T, qos, live && qos >= 0);  // global latency chain, hidden behind the copies issued above
-    cp_async_wait<kStages - 1>();        // the table group is the oldest one
-    __syncthreads();
-    JsonCold cold;  // rarely touched parse state: local memory on purpose (json_engine.cuh)
-    JsonT ev;
-    ev.init(K_RESP, body, stack_words, &cold, tabs);
-    feed_pipe<SCHED>(ev, pipe, 0);
-    if (live) {
-      if (pending) reason = ARKS_R_PENDING;
-      else if (!ev.ok_at_end()) reason = ARKS_R_RESPONSE_UNMARSHAL;   // :157-166
-      else if (cold.m_rawlen == 0) reason = ARKS_R_RESPONSE_UNKNOWN;  // :167-181
-      else { u0 = cold.usage[0]; u1 = cold.usage[1]; u2 = cold.usage[2]; }
-      counted = reason == ARKS_R_OK && u2 != 0;  // :186
-    }
+  __shared__ __align__(16) JsonSmem<true, false> json_smem;
+  pdl_open();
+  const JsonTables tabs = json_smem.stage_async();
+  pdl_wait();  // on every path (see pdl_wait): B.perm, the list and its counter are written by earlier kernels
+  const uint32_t n = FROM_LIST ? *B.slow_n + 1u : B.n;  // the counter starts at -1 (batch_head_kernel clears it)
+  const uint32_t warps = FROM_LIST ? gridDim.x * kWarpsPerBlock : 0u;
+  if (FROM_LIST && ((blockIdx.x * blockDim.x) >> 5) * B.bpw >= n) {  // nothing left for this block
+    cp_async_wait<0>();
+    return;
   }
-  account_usage(T, B, i, live, qos, acct, reason, counted, u0, u1, u2);
+  uint32_t stack_words[kStackWords];  // local memory, touched only beyond 32 levels of nesting
+  for (uint32_t q = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, first = 1;; q += warps, first = 0) {
+    const uint32_t lane_id = q * B.bpw + (threadIdx.x & 31);
+    const bool live = (threadIdx.x & 31) < B.bpw && lane_id < n;
+    const uint32_t i = live ? (FROM_LIST ? B.slow_list[lane_id] : B.perm ? B.perm[lane_id] : lane_id) : 0;  // the body this lane parses
+    uint8_t reason = ARKS_R_OK, counted = 0;
+    long long u0 = 0, u1 = 0, u2 = 0;
+    int32_t qos = 0;
+    QosAcct acct;
+    {
+      const uint8_t* body = B.bodies + (live ? B.body_off[i] : 0);
+      const uint8_t fl = live ? B.flags[i] : ARKS_RESP_END_OF_STREAM;
+      const bool pending = !(fl & ARKS_RESP_END_OF_STREAM);  // more of the body is still to come: handle_response.go:141-149
+      qos = live ? B.qos[i] : 0;
+      const uint32_t len = live && !pending && qos >= 0 ? B.body_len[i] : 0;
+      WindowPipe<kStages> pipe;
+      pipe.start(body, len, smem + (threadIdx.x >> 5) * (kStages * kStageBytes));
+      acct = load_qos_acct(T, qos, live && qos >= 0);  // global latency chain, hidden behind the copies issued above
+      if (first) {  // the whole block runs the first round
+        cp_async_wait<kStages - 1>();  // the table group is the oldest one
+        __syncthreads();
+      }
+      JsonCold cold;  // rarely touched parse state: local memory on purpose (json_engine.cuh)
+      JsonT ev;
+      ev.init(K_RESP, body, stack_words, &cold, tabs);
+      feed_pipe<SCHED>(ev, pipe, 0);
+      if (live) {
+        if (pending) reason = ARKS_R_PENDING;
+        else if (!ev.ok_at_end()) reason = ARKS_R_RESPONSE_UNMARSHAL;   // :157-166
+        else if (cold.m_rawlen == 0) reason = ARKS_R_RESPONSE_UNKNOWN;  // :167-181
+        else { u0 = cold.usage[0]; u1 = cold.usage[1]; u2 = cold.usage[2]; }
+        counted = reason == ARKS_R_OK && u2 != 0;  // :186
+      }
+    }
+    account_usage(T, B, i, live, qos, acct, reason, counted, u0, u1, u2);
+    if (!FROM_LIST || (q + warps) * B.bpw >= n) break;
+  }
 }
 
 // the fast path for complete response bodies: first stage of the two-stage scan (see fast_request_kernel)
@@ -1568,8 +1622,13 @@ template <int WALK>
 __global__ void __launch_bounds__(kFastThreads) fast_response_kernel(DevTables T, RespDev B, int regroup) {
   extern __shared__ __align__(1024) uint8_t smem[];
   FastBlockSmem& sm = *reinterpret_cast<FastBlockSmem*>(smem);
+  pdl_open();
   stage_fast_tables(&sm.tabs, &sm.bar);
+  if (B.perm) pdl_wait();  // the length order is written by the kernels before this one
   const uint32_t base = blockIdx.x * blockDim.x;
+  // The qos entry's accounting shape (config only) is fetched before pass A, whose loads hide its dependent chain. Without
+  // regrouping by structure the thread keeps the document it scans; otherwise it is fetched for the row of the tail below.
+  QosAcct acct = load_qos_acct(T, 0, false);
   {
     const uint32_t own = base + threadIdx.x;
     uint32_t len0 = 0;
@@ -1580,11 +1639,13 @@ __global__ void __launch_bounds__(kFastThreads) fast_response_kernel(DevTables T
     const uint32_t a = fast_block_order(sm, min((len0 + 31) >> 5, 63u), regroup != 0);
     const bool in = base + a < B.n;
     const uint32_t i = in ? (B.perm ? B.perm[base + a] : base + a) : 0;
-    const bool scan = in && (B.flags[i] & ARKS_RESP_END_OF_STREAM) && B.qos[i] >= 0;
+    const int32_t qos = in ? B.qos[i] : -1;
+    if ((regroup & 255) < 2) acct = load_qos_acct(T, qos, qos >= 0);
+    const bool scan = in && (B.flags[i] & ARKS_RESP_END_OF_STREAM) && qos >= 0;
     fast_pass_a(B.bodies + (scan ? B.body_off[i] : 0), scan ? B.body_len[i] : 0u, sm);
     sm.slot[threadIdx.x] = a;
   }
-  if (regroup & 256) return;  // timing experiments only: pass A alone
+  if (regroup & 256) { pdl_wait(); return; }  // timing experiments only: pass A alone
   regroup &= 255;
   uint32_t u = threadIdx.x;
   if (regroup > 1) {
@@ -1603,6 +1664,8 @@ __global__ void __launch_bounds__(kFastThreads) fast_response_kernel(DevTables T
   const bool scan2 = in && !pending && qos >= 0;
   FastOut o;
   const bool accepted = fast_pass_bc<K_RESP, WALK>(scan2, B.bodies + (scan2 ? B.body_off[i] : 0), scan2 ? B.body_len[i] : 0u, sm, u, o);
+  // The scan above overlaps the kernel before; the list and the counters come after it. On every path (see pdl_wait)
+  pdl_wait();
   if (scan2) {
     if (accepted) {
       if (o.m_rawlen == 0) reason = ARKS_R_RESPONSE_UNKNOWN;  // handle_response.go:167-181
@@ -1615,7 +1678,7 @@ __global__ void __launch_bounds__(kFastThreads) fast_response_kernel(DevTables T
   } else if (in && pending) {
     reason = ARKS_R_PENDING;  // :141-149 (a row without a qos entry: account_usage answers ARKS_R_QOS_GONE)
   }
-  const QosAcct acct = load_qos_acct(T, qos, live && qos >= 0);
+  if (regroup > 1) acct = load_qos_acct(T, qos, live && qos >= 0);
   account_usage(T, B, i, live, qos, acct, reason, counted, u0, u1, u2);  // all 32 lanes: warp-aggregated atomics inside
 }
 
@@ -1624,7 +1687,9 @@ template <int WALK>
 __global__ void __launch_bounds__(kFastThreads, 7) fast_response_kernel2(DevTables T, RespDev B, int regroup) {
   extern __shared__ __align__(1024) uint8_t smem[];
   FastSplitSmem& sm = *reinterpret_cast<FastSplitSmem*>(smem);
+  pdl_open();
   stage_fast_tables(&sm.tabs, &sm.bar);
+  pdl_wait();  // on every path (see pdl_wait)
   const uint32_t base = blockIdx.x * kSplitDocs, pair = threadIdx.x >> 1;
   const uint32_t own = base + pair;
   uint32_t len0 = 0;
@@ -1675,8 +1740,9 @@ __global__ void __launch_bounds__(kFastThreads, 7) fast_response_kernel2(DevTabl
 __global__ void __launch_bounds__(kWdWarps * 32) warp_response_kernel(DevTables T, RespDev B) {
   extern __shared__ __align__(1024) uint8_t smem[];
   WdWarpSmem& sm = reinterpret_cast<WdWarpSmem*>(smem)[threadIdx.x >> 5];
+  pdl_open();
   const uint32_t i = blockIdx.x * kWdWarps + (threadIdx.x >> 5);
-  if (i >= B.n) return;
+  if (i >= B.n) { pdl_wait(); return; }  // on every path (see pdl_wait)
   const uint32_t lane = threadIdx.x & 31;
   const int32_t qos = B.qos[i];
   const bool pending = !(B.flags[i] & ARKS_RESP_END_OF_STREAM);
@@ -1687,9 +1753,11 @@ __global__ void __launch_bounds__(kWdWarps * 32) warp_response_kernel(DevTables 
   const bool scan = !pending && qos >= 0;
   const bool elig = wd_fetch(sm, B.bodies + B.body_off[i], scan ? len : 0u);
   const QosAcct acct = load_qos_acct(T, qos, live && qos >= 0);  // behind the bulk copy
+  wd::FastOut o;
+  const bool ok = scan && elig && wd_scan_doc<K_RESP>(sm.doc, len, sm, o);
+  pdl_wait();  // the scan above overlaps the kernel before; the list and the counters come after it
   if (scan) {
-    wd::FastOut o;
-    if (elig && wd_scan_doc<K_RESP>(sm.doc, len, sm, o)) {
+    if (ok) {
       if (o.m_rawlen == 0) reason = ARKS_R_RESPONSE_UNKNOWN;  // handle_response.go:167-181
       else { u0 = o.usage[0]; u1 = o.usage[1]; u2 = o.usage[2]; }
       counted = reason == ARKS_R_OK && u2 != 0;               // :186
@@ -1722,12 +1790,14 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32, ARKS_SSE_MINBLK) scan_sse
   __shared__ uint2 s_desc[kWarpsPerBlock][kSseEvCap];  // x: byte offset of the payload in B.bodies; y: len | owner<<16 | seq<<21
   __shared__ long long s_usage[kWarpsPerBlock][32][3];
   __shared__ uint32_t s_best[kWarpsPerBlock][32], s_fail[kWarpsPerBlock][32], s_n[kWarpsPerBlock];
+  pdl_open();
+  const JsonTables tabs = json_smem.stage_async();
+  pdl_wait();  // on every path (see pdl_wait): B.perm is written by earlier kernels
   const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const uint32_t lane_id = ((blockIdx.x * blockDim.x + threadIdx.x) >> 5) * B.bpw + lane;
   const bool live = lane < B.bpw && lane_id < B.n;
   const uint32_t i = live ? (B.perm ? B.perm[lane_id] : lane_id) : 0;  // the chunk this lane cuts and accounts
   uint8_t* wsmem = smem + warp * (kSseStages * kStageBytes);
-  const JsonTables tabs = json_smem.stage_async();
   const uint32_t chunk_off = live ? B.body_off[i] : 0;
   const int32_t qos = live ? B.qos[i] : 0;
   const uint32_t len = live && qos >= 0 ? B.body_len[i] : 0;
@@ -1833,6 +1903,8 @@ __global__ void __launch_bounds__(128) bpe_scan_kernel(const uint8_t* bodies, co
                                                        BpeTablesDev T, uint8_t* text, unsigned long long* list, uint32_t* list_n,
                                                        uint32_t list_cap, uint32_t* bpe_out, const uint8_t* row_flags, uint32_t wide_mask,
                                                        const uint32_t* rows, const uint32_t* rows_n) {
+  pdl_open();
+  pdl_wait();  // on every path (see pdl_wait)
   const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= (kRows ? *rows_n : n)) return;
   const uint32_t i = kRows ? rows[k] : k;
@@ -1871,6 +1943,7 @@ __global__ void __launch_bounds__(kBpeMergeThreads) bpe_merge_kernel(const unsig
                                                                     BpeTablesDev T, const uint8_t* text, uint32_t* bpe_out) {
   __shared__ __align__(128) BpeSlot hot[kBpeHotSlots];
   __shared__ uint64_t bar;
+  pdl_open();
   if (threadIdx.x == 0) {
     mbar_init(&bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -1879,6 +1952,7 @@ __global__ void __launch_bounds__(kBpeMergeThreads) bpe_merge_kernel(const unsig
   }
   __syncthreads();
   mbar_wait(&bar, 0);
+  pdl_wait();  // on every path (see pdl_wait): the list is written by the scan kernel before this one
   const uint32_t total = min(*list_n, list_cap);
   for (uint32_t k = blockIdx.x * blockDim.x + threadIdx.x; k < total; k += gridDim.x * blockDim.x) {
     const unsigned long long e = list[k];
@@ -1894,6 +1968,8 @@ __global__ void __launch_bounds__(kBpeMergeThreads) bpe_merge_kernel(const unsig
 // their lengths (zeroed before). One atomic per distinct slot per warp.
 __global__ void __launch_bounds__(128) bpe_split_kernel(const uint8_t* qos_vocab, const int32_t* qos_of, uint32_t n, uint32_t loaded,
                                                         uint32_t* rows, uint32_t stride, uint32_t* rows_n) {
+  pdl_open();
+  pdl_wait();  // on every path (see pdl_wait)
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const int32_t q = qos_of[i];
@@ -1915,6 +1991,8 @@ __global__ void __launch_bounds__(128) bpe_split_kernel(const uint8_t* qos_vocab
 // 1: completion chunks (quota item response, gateway_token_usage{output}); tpm / tpd and quota item total on both.
 __global__ void __launch_bounds__(128) meter_charge_kernel(DevTables T, uint32_t n, const uint8_t* reason, const uint8_t* flags, uint32_t mask,
                                                            const int32_t* qos_of, const uint32_t* bpe, const uint32_t* body_len, int side) {
+  pdl_open();
+  pdl_wait();  // on every path (see pdl_wait)
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   bool on = i < n && reason[i] == ARKS_R_OK && (flags[i] & mask) == mask;
   const int32_t qos = on ? qos_of[i] : -1;
@@ -2155,6 +2233,25 @@ static int64_t window_start(int64_t now, int rule) {            // ratelimiter/c
 }
 
 static size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
+
+// Launch one kernel of a batch's chain on the compute stream with programmatic dependent launch: the grid may start while
+// the kernel before it drains, and passes its pdl_wait() once that kernel has completed. A copy, memset or event wait in
+// front of it is an ordinary stream dependency and still completes first. Launch errors surface at the run's
+// cudaGetLastError().
+template <typename... P, typename... A>
+static void launch_chained(arks_ctx* ctx, void (*kernel)(P...), dim3 grid, dim3 block, size_t smem, A&&... args) {
+  cudaLaunchAttribute attr;
+  attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr.val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = grid;
+  cfg.blockDim = block;
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = ctx->stream;
+  cfg.attrs = &attr;
+  cfg.numAttrs = 1;
+  cudaLaunchKernelEx(&cfg, kernel, std::forward<A>(args)...);
+}
 
 extern "C" {
 
@@ -2517,18 +2614,18 @@ static int queue_bpe(arks_ctx* ctx, const uint8_t* bodies, const uint32_t* body_
     const BpeTablesDev& T = ctx->bpe[0];
     CK(cudaMemsetAsync(ctx->d_bpe_n, 0, 4, ctx->stream));
     if (T.flags & ARKS_BPE_DIGITS3)
-      bpe_scan_kernel<3, false><<<(n + 127) / 128, 128, 0, ctx->stream>>>(bodies, body_off, body_len, n, T, ctx->d_bpe_text, ctx->d_bpe_list,
+      launch_chained(ctx, bpe_scan_kernel<3, false>, (n + 127) / 128, 128, 0, bodies, body_off, body_len, n, T, ctx->d_bpe_text, ctx->d_bpe_list,
                                                                           ctx->d_bpe_n, ctx->bpe_list_cap, bpe_out, row_flags, wide_mask,
                                                                           nullptr, nullptr);
     else
-      bpe_scan_kernel<1, false><<<(n + 127) / 128, 128, 0, ctx->stream>>>(bodies, body_off, body_len, n, T, ctx->d_bpe_text, ctx->d_bpe_list,
+      launch_chained(ctx, bpe_scan_kernel<1, false>, (n + 127) / 128, 128, 0, bodies, body_off, body_len, n, T, ctx->d_bpe_text, ctx->d_bpe_list,
                                                                           ctx->d_bpe_n, ctx->bpe_list_cap, bpe_out, row_flags, wide_mask,
                                                                           nullptr, nullptr);
     if (T.flags & ARKS_BPE_IGNORE_MERGES)
-      bpe_merge_kernel<true><<<ctx->n_sm * 4, kBpeMergeThreads, 0, ctx->stream>>>(ctx->d_bpe_list, ctx->d_bpe_n, ctx->bpe_list_cap, T,
+      launch_chained(ctx, bpe_merge_kernel<true>, ctx->n_sm * 4, kBpeMergeThreads, 0, ctx->d_bpe_list, ctx->d_bpe_n, ctx->bpe_list_cap, T,
                                                                                   ctx->d_bpe_text, bpe_out);
     else
-      bpe_merge_kernel<false><<<ctx->n_sm * 4, kBpeMergeThreads, 0, ctx->stream>>>(ctx->d_bpe_list, ctx->d_bpe_n, ctx->bpe_list_cap, T,
+      launch_chained(ctx, bpe_merge_kernel<false>, ctx->n_sm * 4, kBpeMergeThreads, 0, ctx->d_bpe_list, ctx->d_bpe_n, ctx->bpe_list_cap, T,
                                                                                    ctx->d_bpe_text, bpe_out);
     ctx->launches += 2;
     return 0;
@@ -2541,25 +2638,25 @@ static int queue_bpe(arks_ctx* ctx, const uint8_t* bodies, const uint32_t* body_
   uint32_t* rows_n = ctx->d_bpe_n + 32;
   const uint32_t use = (ctx->vocab_used | 1u) & ctx->vocab_loaded;
   CK(cudaMemsetAsync(list_n, 0, 32 * 4, ctx->stream));
-  bpe_split_kernel<<<(n + 127) / 128, 128, 0, ctx->stream>>>(ctx->dt.qos_vocab, row_qos, n, use, ctx->d_bpe_rows, ctx->max_batch, rows_n);
+  launch_chained(ctx, bpe_split_kernel, (n + 127) / 128, 128, 0, ctx->dt.qos_vocab, row_qos, n, use, ctx->d_bpe_rows, ctx->max_batch, rows_n);
   ctx->launches += 1;
   for (uint32_t v = 0; v < kBpeMaxVocabs; v++) {
     if (!((use >> v) & 1u)) continue;
     const BpeTablesDev& T = ctx->bpe[v];
     const uint32_t* rows = ctx->d_bpe_rows + (size_t)v * ctx->max_batch;
     if (T.flags & ARKS_BPE_DIGITS3)
-      bpe_scan_kernel<3, true><<<(n + 127) / 128, 128, 0, ctx->stream>>>(bodies, body_off, body_len, n, T, ctx->d_bpe_text, ctx->d_bpe_list,
+      launch_chained(ctx, bpe_scan_kernel<3, true>, (n + 127) / 128, 128, 0, bodies, body_off, body_len, n, T, ctx->d_bpe_text, ctx->d_bpe_list,
                                                                          list_n + v, ctx->bpe_list_cap, bpe_out, row_flags, wide_mask, rows,
                                                                          rows_n + v);
     else
-      bpe_scan_kernel<1, true><<<(n + 127) / 128, 128, 0, ctx->stream>>>(bodies, body_off, body_len, n, T, ctx->d_bpe_text, ctx->d_bpe_list,
+      launch_chained(ctx, bpe_scan_kernel<1, true>, (n + 127) / 128, 128, 0, bodies, body_off, body_len, n, T, ctx->d_bpe_text, ctx->d_bpe_list,
                                                                          list_n + v, ctx->bpe_list_cap, bpe_out, row_flags, wide_mask, rows,
                                                                          rows_n + v);
     if (T.flags & ARKS_BPE_IGNORE_MERGES)
-      bpe_merge_kernel<true><<<ctx->n_sm * 4, kBpeMergeThreads, 0, ctx->stream>>>(ctx->d_bpe_list, list_n + v, ctx->bpe_list_cap, T,
+      launch_chained(ctx, bpe_merge_kernel<true>, ctx->n_sm * 4, kBpeMergeThreads, 0, ctx->d_bpe_list, list_n + v, ctx->bpe_list_cap, T,
                                                                                   ctx->d_bpe_text, bpe_out);
     else
-      bpe_merge_kernel<false><<<ctx->n_sm * 4, kBpeMergeThreads, 0, ctx->stream>>>(ctx->d_bpe_list, list_n + v, ctx->bpe_list_cap, T,
+      launch_chained(ctx, bpe_merge_kernel<false>, ctx->n_sm * 4, kBpeMergeThreads, 0, ctx->d_bpe_list, list_n + v, ctx->bpe_list_cap, T,
                                                                                    ctx->d_bpe_text, bpe_out);
     ctx->launches += 2;
   }
@@ -2569,7 +2666,7 @@ static int queue_bpe(arks_ctx* ctx, const uint8_t* bodies, const uint32_t* body_
 static int queue_meter(arks_ctx* ctx, uint32_t n, const uint8_t* reason, const uint8_t* flags, uint32_t mask, const int32_t* qos,
                        const uint32_t* bpe, const uint32_t* body_len, int side) {
   if (ctx->prof) CK(cudaEventRecord(ctx->ev_meter[0], ctx->stream));
-  meter_charge_kernel<<<(n + 127) / 128, 128, 0, ctx->stream>>>(ctx->dt, n, reason, flags, mask, qos, bpe, body_len, side);
+  launch_chained(ctx, meter_charge_kernel, (n + 127) / 128, 128, 0, ctx->dt, n, reason, flags, mask, qos, bpe, body_len, side);
   if (ctx->prof) { CK(cudaEventRecord(ctx->ev_meter[1], ctx->stream)); ctx->ev_meter_set = true; }
   ctx->launches += 1;
   return 0;
@@ -3021,9 +3118,10 @@ int arks_update_endpoint_weights(arks_ctx* ctx, uint32_t ep, uint32_t n, const i
 // becomes the previous one (plane 4 + rule) when the new one follows it directly; when time skipped a window the previous
 // plane is marked stale instead (prev_ok: reads as 0) rather than cleared. Kept whether or not the sliding window is on, so
 // that switching it on at any batch is exact. Rules that roll together are handled as one span of planes: one copy (a
-// skipped rule's plane inside it is copied too and marked stale) and one memset, so a roll-over of every rule queues two
-// operations, no kernel
-static int roll_windows(arks_ctx* ctx, int64_t now) {
+// skipped rule's plane inside it is copied too and marked stale) and one clear. This only decides: bit r of *roll is a
+// plane to clear, bit r of *keep one to copy to plane 4 + r first, and batch_head_kernel does both on the device.
+static int roll_windows(arks_ctx* ctx, int64_t now, uint32_t* roll, uint32_t* keep) {
+  *roll = *keep = 0;
   for (int r = 0; r < 4; r++)
     if (window_start(now, r) < ctx->last_win[r])
       return fail(ctx, ARKS_E_TIME_WENT_BACK, "now_unix %lld is before the current %s window", (long long)now,
@@ -3037,19 +3135,47 @@ static int roll_windows(arks_ctx* ctx, int64_t now) {
       ctx->last_win[r] = ws;
     }
   }
-  const size_t nq = ctx->ht.n_qos;
   for (int a = 0; a < 4;) {
     if (!rolled[a]) { a++; continue; }
     int b = a;
     bool copy = false;
     for (; b < 4 && rolled[b]; b++) copy |= adjacent[b];
-    if (nq && copy) CK(cudaMemcpyAsync(ctx->d_rate + (size_t)(4 + a) * nq, ctx->d_rate + (size_t)a * nq, 8 * nq * (b - a),
-                                       cudaMemcpyDeviceToDevice, ctx->stream));
-    if (nq) CK(cudaMemsetAsync(ctx->d_rate + (size_t)a * nq, 0, 8 * nq * (b - a), ctx->stream));
-    for (int r = a; r < b; r++) ctx->prev_ok = adjacent[r] ? ctx->prev_ok | 1u << r : ctx->prev_ok & ~(1u << r);
+    for (int r = a; r < b; r++) {
+      *roll |= 1u << r;
+      if (copy) *keep |= 1u << r;
+      ctx->prev_ok = adjacent[r] ? ctx->prev_ok | 1u << r : ctx->prev_ok & ~(1u << r);
+    }
     a = b;
   }
   return 0;
+}
+
+// The first kernel of every request and response run, so that no copy or memset sits between the kernels of the chain:
+// the window roll roll_windows() decided (plane r of `roll` copied to plane 4 + r when `keep` has r too, then zeroed), then
+// `nset` words at `set` to -1 (request: the group table and the hot-group and declined-row counters; response: the
+// declined-row counter) and `nzero` words at `zero` to 0 (a response's BPE counts when no vocabulary counts them).
+__global__ void __launch_bounds__(256) batch_head_kernel(long long* rate, uint32_t nq, uint32_t roll, uint32_t keep, int32_t* set,
+                                                         uint32_t nset, uint32_t* zero, uint32_t nzero) {
+  pdl_open();
+  pdl_wait();  // before any write, on every path (see pdl_wait)
+  const uint32_t t0 = blockIdx.x * blockDim.x + threadIdx.x, stride = gridDim.x * blockDim.x;
+  for (int r = 0; r < 4; r++) {
+    if (!(roll >> r & 1u)) continue;
+    long long* cur = rate + (size_t)r * nq;
+    long long* prev = rate + (size_t)(4 + r) * nq;
+    for (uint32_t j = t0; j < nq; j += stride) {
+      if (keep >> r & 1u) prev[j] = cur[j];
+      cur[j] = 0;
+    }
+  }
+  for (uint32_t j = t0; j < nset; j += stride) set[j] = -1;
+  for (uint32_t j = t0; j < nzero; j += stride) zero[j] = 0;
+}
+static void queue_head(arks_ctx* ctx, uint32_t roll, uint32_t keep, int32_t* set, uint32_t nset, uint32_t* zero, uint32_t nzero) {
+  const uint32_t nq = ctx->ht.n_qos, words = std::max(roll ? nq : 0u, std::max(nset, nzero));
+  const uint32_t grid = std::min((words + 1023) / 1024 + 1, (uint32_t)ctx->n_sm * 4);  // about four words per thread
+  launch_chained(ctx, batch_head_kernel, grid, 256, 0, ctx->d_rate, nq, roll, keep, set, nset, zero, nzero);
+  ctx->launches += 1;
 }
 
 // ---- staging slots --------------------------------------------------------------------------------
@@ -3240,6 +3366,11 @@ static uint32_t bodies_per_warp(uint32_t n) {
   return b < 1 ? 1 : b > 32 ? 32 : b;
 }
 static uint32_t scan_grid(uint32_t n, uint32_t bpw) { return ((n + bpw - 1) / bpw + kWarpsPerBlock - 1) / kWarpsPerBlock; }
+// The declined-row pass (FROM_LIST) is queued before its list is known: at most the blocks that are resident at once, whose
+// warps stride over the list. An empty list costs one wave of blocks that exit at once, however large the batch.
+static uint32_t scan_list_grid(const arks_ctx* ctx, uint32_t n, uint32_t bpw) {
+  return std::min(scan_grid(n, bpw), (uint32_t)(ctx->n_sm * kMinBlocks));
+}
 
 // batches below this size are a handful of warps: the three small launches would cost more than they save
 constexpr uint32_t kSortMinBatch = 4096;
@@ -3251,9 +3382,9 @@ constexpr uint32_t kSortMinBatch = 4096;
 static const uint32_t* queue_length_order(arks_ctx* ctx, const uint32_t* d_body_len, uint32_t n) {
   if (!ctx->sort_lanes || n < kSortMinBatch) return nullptr;
   cudaMemsetAsync(ctx->d_lenhist, 0, (size_t)4 * kLenBuckets, ctx->stream);
-  len_hist_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(d_body_len, n, ctx->d_lenhist);
-  len_scan_kernel<<<1, 1024, 0, ctx->stream>>>(ctx->d_lenhist);
-  len_scatter_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(d_body_len, n, ctx->d_lenhist, ctx->d_perm);
+  launch_chained(ctx, len_hist_kernel, (n + 255) / 256, 256, 0, d_body_len, n, ctx->d_lenhist);
+  launch_chained(ctx, len_scan_kernel, 1, 1024, 0, ctx->d_lenhist);
+  launch_chained(ctx, len_scatter_kernel, (n + 255) / 256, 256, 0, d_body_len, n, ctx->d_lenhist, ctx->d_perm);
   ctx->launches += 3;
   return ctx->d_perm;
 }
@@ -3263,7 +3394,8 @@ int arks_run_request_batch(arks_ctx* ctx, int64_t now_unix) {
   arks_ctx::Slot& sl = ctx->slots[ctx->cur];
   if (!sl.req_staged) return fail(ctx, ARKS_E_INVALID_ARG, "no request batch staged in slot %d", ctx->cur);
   CK(cudaSetDevice(ctx->device));
-  int rc = roll_windows(ctx, now_unix);
+  uint32_t roll, keep;
+  int rc = roll_windows(ctx, now_unix, &roll, &keep);
   if (rc) return rc;
   const uint32_t n = sl.req_n;
   ctx->fetch_n = n;
@@ -3272,7 +3404,11 @@ int arks_run_request_batch(arks_ctx* ctx, int64_t now_unix) {
   ctx->ev_bpe_set = false;
   ctx->ev_meter_set = false;
   ctx->last_two_stage = false;
-  if (n == 0) return 0;
+  if (n == 0) {
+    queue_head(ctx, roll, keep, nullptr, 0, nullptr, 0);
+    CK(cudaGetLastError());
+    return 0;
+  }
   CK(cudaStreamWaitEvent(ctx->stream, sl.req_copied, 0));
   ReqDev& r = sl.rq;
   sl.req_zc = n <= kZeroCopyRows && sl.h_req_result;
@@ -3287,23 +3423,23 @@ int arks_run_request_batch(arks_ctx* ctx, int64_t now_unix) {
   uint32_t g = 64;
   while (g < 2 * n) g <<= 1;
   r.gmask = g - 1;
-  // gkey | ghead | gcnt are laid out back to back for THIS batch's table size: one memset(0xff) clears all three
+  // gkey | ghead | gcnt are laid out back to back for THIS batch's table size: the head kernel clears all three to -1
   r.ghead = r.gkey + g;
   r.gcnt = r.gkey + 2 * (size_t)g;
   r.hot_n = r.gkey + 3 * (size_t)g;  // one more word: the hot-group counter, also starting at -1
-  CK(cudaMemsetAsync(r.gkey, 0xff, (size_t)g * 12 + 8, ctx->stream));  // + the hot-group and declined-rows counters
+  queue_head(ctx, roll, keep, r.gkey, g * 3 + 2, nullptr, 0);  // + the hot-group and declined-rows counters
   const uint32_t tpb = kWarpsPerBlock * 32;
-  r.slow_n = reinterpret_cast<uint32_t*>(r.hot_n + 1);  // cleared to -1 by the group table's memset
+  r.slow_n = reinterpret_cast<uint32_t*>(r.hot_n + 1);  // cleared to -1 with the group table
   r.slow_list = ctx->d_slow + 64;
   ctx->last_slow_n = r.slow_n;
   if (ctx->prof) CK(cudaEventRecord(ctx->ev[0], ctx->stream));
   if (ctx->fast_scan && n <= ctx->warp_max) {
     // latency path: a warp per body (warp_scan.cuh), the exact engine for what it declines
     r.perm = nullptr;
-    warp_request_kernel<<<(n + kWdWarps - 1) / kWdWarps, kWdWarps * 32, kWdSmemPerBlock, ctx->stream>>>(ctx->dt, r);
+    launch_chained(ctx, warp_request_kernel, (n + kWdWarps - 1) / kWdWarps, kWdWarps * 32, kWdSmemPerBlock, ctx->dt, r);
     r.bpw = 1;
     switch (ctx->sched[0]) {
-#define ARKS_LAUNCH(S) case S: scan_request_kernel<S, true><<<scan_grid(n, r.bpw), tpb, kSmemPerBlock, ctx->stream>>>(ctx->dt, r); break;
+#define ARKS_LAUNCH(S) case S: launch_chained(ctx, scan_request_kernel<S, true>, scan_list_grid(ctx, n, r.bpw), tpb, kSmemPerBlock, ctx->dt, r); break;
       ARKS_FOR_SCHED(ARKS_LAUNCH)
 #undef ARKS_LAUNCH
     }
@@ -3316,16 +3452,16 @@ int arks_run_request_batch(arks_ctx* ctx, int64_t now_unix) {
     r.perm = ctx->sort_fast ? queue_length_order(ctx, r.body_len, n) : nullptr;
     if (ctx->prof) CK(cudaEventRecord(ctx->ev_fast[0], ctx->stream));
     if (ctx->split)
-      fast_request_kernel2<8><<<(n + kSplitDocs - 1) / kSplitDocs, kFastThreads, sizeof(FastSplitSmem), ctx->stream>>>(ctx->dt, r, ctx->regroup);
+      launch_chained(ctx, fast_request_kernel2<8>, (n + kSplitDocs - 1) / kSplitDocs, kFastThreads, sizeof(FastSplitSmem), ctx->dt, r, ctx->regroup);
     else if (ctx->walk8)
-      fast_request_kernel<8><<<(n + kFastThreads - 1) / kFastThreads, kFastThreads, sizeof(FastBlockSmem), ctx->stream>>>(ctx->dt, r, ctx->regroup);
+      launch_chained(ctx, fast_request_kernel<8>, (n + kFastThreads - 1) / kFastThreads, kFastThreads, sizeof(FastBlockSmem), ctx->dt, r, ctx->regroup);
     else
-      fast_request_kernel<0><<<(n + kFastThreads - 1) / kFastThreads, kFastThreads, sizeof(FastBlockSmem), ctx->stream>>>(ctx->dt, r, ctx->regroup);
+      launch_chained(ctx, fast_request_kernel<0>, (n + kFastThreads - 1) / kFastThreads, kFastThreads, sizeof(FastBlockSmem), ctx->dt, r, ctx->regroup);
     if (ctx->prof) { CK(cudaEventRecord(ctx->ev_fast[1], ctx->stream)); ctx->ev_fast_set = true; }
     r.perm = nullptr;
     r.bpw = 32;
     switch (ctx->sched[0]) {
-#define ARKS_LAUNCH(S) case S: scan_request_kernel<S, true><<<scan_grid(n, r.bpw), tpb, kSmemPerBlock, ctx->stream>>>(ctx->dt, r); break;
+#define ARKS_LAUNCH(S) case S: launch_chained(ctx, scan_request_kernel<S, true>, scan_list_grid(ctx, n, r.bpw), tpb, kSmemPerBlock, ctx->dt, r); break;
       ARKS_FOR_SCHED(ARKS_LAUNCH)
 #undef ARKS_LAUNCH
     }
@@ -3335,7 +3471,7 @@ int arks_run_request_batch(arks_ctx* ctx, int64_t now_unix) {
     r.perm = queue_length_order(ctx, r.body_len, n);
     r.bpw = bodies_per_warp(n);
     switch (ctx->sched[0]) {
-#define ARKS_LAUNCH(S) case S: scan_request_kernel<S, false><<<scan_grid(n, r.bpw), tpb, kSmemPerBlock, ctx->stream>>>(ctx->dt, r); break;
+#define ARKS_LAUNCH(S) case S: launch_chained(ctx, scan_request_kernel<S, false>, scan_grid(n, r.bpw), tpb, kSmemPerBlock, ctx->dt, r); break;
       ARKS_FOR_SCHED(ARKS_LAUNCH)
 #undef ARKS_LAUNCH
     }
@@ -3349,11 +3485,11 @@ int arks_run_request_batch(arks_ctx* ctx, int64_t now_unix) {
   }
   if (ctx->prof) CK(cudaEventRecord(ctx->ev_admit0, ctx->stream));
   if (n > (uint32_t)kHotGroup) {  // a group can only be hot if the batch is larger than the threshold
-    rank_hot_groups_kernel<<<296, 256, 0, ctx->stream>>>(r);  // exits at once when scan_request listed no hot group
+    launch_chained(ctx, rank_hot_groups_kernel, 296, 256, 0, r);  // exits at once when scan_request listed no hot group
     ctx->launches += 1;
   }
   r.precharge = ctx->precharge && ctx->bpe_on ? 1 : 0;
-  limit_admit_kernel<<<(n + 127) / 128, 128, 0, ctx->stream>>>(ctx->dt, r);
+  launch_chained(ctx, limit_admit_kernel, (n + 127) / 128, 128, 0, ctx->dt, r);
   if (ctx->prof) { CK(cudaEventRecord(ctx->ev[2], ctx->stream)); ctx->ev_n = 3; ctx->is_req_timing = true; }
   if (ctx->meter) {  // N5: the prompts of the admitted metered rows are charged when the micro-batch commits
     rc = queue_meter(ctx, n, r.reason, r.flags, ARKS_FLAG_METERED, r.qos, ctx->bpe_on ? r.bpe : nullptr, r.body_len, 0);
@@ -3553,7 +3689,8 @@ int arks_run_response_batch(arks_ctx* ctx, int64_t now_unix) {
   arks_ctx::Slot& sl = ctx->slots[ctx->cur];
   if (!sl.resp_staged) return fail(ctx, ARKS_E_INVALID_ARG, "no response batch staged in slot %d", ctx->cur);
   CK(cudaSetDevice(ctx->device));
-  int rc = roll_windows(ctx, now_unix);
+  uint32_t roll, keep;
+  int rc = roll_windows(ctx, now_unix, &roll, &keep);
   if (rc) return rc;
   const uint32_t n = sl.resp_n;
   ctx->fetch_n = n;
@@ -3562,9 +3699,18 @@ int arks_run_response_batch(arks_ctx* ctx, int64_t now_unix) {
   ctx->ev_bpe_set = false;
   ctx->ev_meter_set = false;
   ctx->last_two_stage = false;
-  if (n == 0) return 0;
+  if (n == 0) {
+    queue_head(ctx, roll, keep, nullptr, 0, nullptr, 0);
+    CK(cudaGetLastError());
+    return 0;
+  }
   const uint32_t tpb = kWarpsPerBlock * 32;
   CK(cudaStreamWaitEvent(ctx->stream, sl.resp_copied, 0));
+  // complete bodies take the warp-per-body latency path or the two-stage scan, both of which list the rows they decline
+  const bool warp_path = sl.resp_mode == 1 && ctx->fast_scan && n <= ctx->warp_max;
+  const bool two_stage = warp_path || (sl.resp_mode == 1 && ctx->fast_scan && n >= ctx->fast_min);
+  queue_head(ctx, roll, keep, two_stage ? reinterpret_cast<int32_t*>(ctx->d_slow) : nullptr, two_stage ? 1 : 0,
+             ctx->bpe_on ? nullptr : sl.rp.bpe, ctx->bpe_on ? 0 : n);
   if (ctx->prof) CK(cudaEventRecord(ctx->ev[0], ctx->stream));
   // complete bodies and SSE chunks have their own kernels; a mixed batch is two launches over the two halves of its
   // kind index (arrival order inside a kind), a homogeneous one a single launch in length order
@@ -3572,7 +3718,7 @@ int arks_run_response_batch(arks_ctx* ctx, int64_t now_unix) {
     rp.bpw = bodies_per_warp(rp.n);
     const dim3 grid(scan_grid(rp.n, rp.bpw));
     switch (ctx->sched[1]) {
-#define ARKS_LAUNCH(S) case S: scan_response_kernel<S, false><<<grid, tpb, kSmemPerBlock, ctx->stream>>>(ctx->dt, rp); break;
+#define ARKS_LAUNCH(S) case S: launch_chained(ctx, scan_response_kernel<S, false>, grid, tpb, kSmemPerBlock, ctx->dt, rp); break;
       ARKS_FOR_SCHED(ARKS_LAUNCH)
 #undef ARKS_LAUNCH
     }
@@ -3581,21 +3727,20 @@ int arks_run_response_batch(arks_ctx* ctx, int64_t now_unix) {
     rp.slow_n = ctx->d_slow;
     rp.slow_list = ctx->d_slow + 64;
     ctx->last_slow_n = rp.slow_n;
-    CK(cudaMemsetAsync(ctx->d_slow, 0xff, 4, ctx->stream));
     rp.perm = ctx->sort_fast ? queue_length_order(ctx, rp.body_len, rp.n) : nullptr;
     if (ctx->prof) CK(cudaEventRecord(ctx->ev_fast[0], ctx->stream));
     if (ctx->split)
-      fast_response_kernel2<8><<<(rp.n + kSplitDocs - 1) / kSplitDocs, kFastThreads, sizeof(FastSplitSmem), ctx->stream>>>(ctx->dt, rp, ctx->regroup);
+      launch_chained(ctx, fast_response_kernel2<8>, (rp.n + kSplitDocs - 1) / kSplitDocs, kFastThreads, sizeof(FastSplitSmem), ctx->dt, rp, ctx->regroup);
     else if (ctx->walk8)
-      fast_response_kernel<8><<<(rp.n + kFastThreads - 1) / kFastThreads, kFastThreads, sizeof(FastBlockSmem), ctx->stream>>>(ctx->dt, rp, ctx->regroup);
+      launch_chained(ctx, fast_response_kernel<8>, (rp.n + kFastThreads - 1) / kFastThreads, kFastThreads, sizeof(FastBlockSmem), ctx->dt, rp, ctx->regroup);
     else
-      fast_response_kernel<0><<<(rp.n + kFastThreads - 1) / kFastThreads, kFastThreads, sizeof(FastBlockSmem), ctx->stream>>>(ctx->dt, rp, ctx->regroup);
+      launch_chained(ctx, fast_response_kernel<0>, (rp.n + kFastThreads - 1) / kFastThreads, kFastThreads, sizeof(FastBlockSmem), ctx->dt, rp, ctx->regroup);
     if (ctx->prof) { CK(cudaEventRecord(ctx->ev_fast[1], ctx->stream)); ctx->ev_fast_set = true; }
     rp.perm = nullptr;
     rp.bpw = 32;
-    const dim3 grid(scan_grid(rp.n, rp.bpw));
+    const dim3 grid(scan_list_grid(ctx, rp.n, rp.bpw));
     switch (ctx->sched[1]) {
-#define ARKS_LAUNCH(S) case S: scan_response_kernel<S, true><<<grid, tpb, kSmemPerBlock, ctx->stream>>>(ctx->dt, rp); break;
+#define ARKS_LAUNCH(S) case S: launch_chained(ctx, scan_response_kernel<S, true>, grid, tpb, kSmemPerBlock, ctx->dt, rp); break;
       ARKS_FOR_SCHED(ARKS_LAUNCH)
 #undef ARKS_LAUNCH
     }
@@ -3607,7 +3752,7 @@ int arks_run_response_batch(arks_ctx* ctx, int64_t now_unix) {
     rp.bpw = bodies_per_warp(rp.n);
     const dim3 grid(scan_grid(rp.n, rp.bpw));
     switch (ctx->sched[2]) {
-#define ARKS_LAUNCH(S) case S: scan_sse_kernel<S><<<grid, tpb, kSseSmemPerBlock, ctx->stream>>>(ctx->dt, rp); break;
+#define ARKS_LAUNCH(S) case S: launch_chained(ctx, scan_sse_kernel<S>, grid, tpb, kSseSmemPerBlock, ctx->dt, rp); break;
       ARKS_FOR_SCHED(ARKS_LAUNCH)
 #undef ARKS_LAUNCH
     }
@@ -3620,24 +3765,23 @@ int arks_run_response_batch(arks_ctx* ctx, int64_t now_unix) {
     launch_sse(rs);
     ctx->launches += 1;
   } else {
-    if (sl.resp_mode == 1 && ctx->fast_scan && n <= ctx->warp_max) {
+    if (warp_path) {
       RespDev rp = sl.rp;
       rp.slow_n = ctx->d_slow;
       rp.slow_list = ctx->d_slow + 64;
       rp.perm = nullptr;
       ctx->last_slow_n = rp.slow_n;
-      CK(cudaMemsetAsync(ctx->d_slow, 0xff, 4, ctx->stream));
-      warp_response_kernel<<<(n + kWdWarps - 1) / kWdWarps, kWdWarps * 32, kWdSmemPerBlock, ctx->stream>>>(ctx->dt, rp);
+      launch_chained(ctx, warp_response_kernel, (n + kWdWarps - 1) / kWdWarps, kWdWarps * 32, kWdSmemPerBlock, ctx->dt, rp);
       rp.bpw = 1;
-      const dim3 grid(scan_grid(n, rp.bpw));
+      const dim3 grid(scan_list_grid(ctx, n, rp.bpw));
       switch (ctx->sched[1]) {
-#define ARKS_LAUNCH(S) case S: scan_response_kernel<S, true><<<grid, tpb, kSmemPerBlock, ctx->stream>>>(ctx->dt, rp); break;
+#define ARKS_LAUNCH(S) case S: launch_chained(ctx, scan_response_kernel<S, true>, grid, tpb, kSmemPerBlock, ctx->dt, rp); break;
         ARKS_FOR_SCHED(ARKS_LAUNCH)
 #undef ARKS_LAUNCH
       }
       ctx->launches += 1;
       ctx->last_two_stage = true;
-    } else if (sl.resp_mode == 1 && ctx->fast_scan && n >= ctx->fast_min) {
+    } else if (two_stage) {
       rc = launch_json_two_stage(sl.rp);
       if (rc) return rc;
     } else {
@@ -3652,8 +3796,6 @@ int arks_run_response_batch(arks_ctx* ctx, int64_t now_unix) {
                    ARKS_RESP_STREAM | ARKS_RESP_METERED, sl.rp.qos);
     if (rc) return rc;
     if (ctx->prof) { CK(cudaEventRecord(ctx->ev_bpe[1], ctx->stream)); ctx->ev_bpe_set = true; }
-  } else {
-    CK(cudaMemsetAsync(sl.rp.bpe, 0, (size_t)n * 4, ctx->stream));
   }
   if (sl.resp_metered) {  // N5: metered chunks answered ARKS_R_OK are billed their completion count
     rc = queue_meter(ctx, n, sl.rp.reason, sl.rp.flags, ARKS_RESP_STREAM | ARKS_RESP_METERED, sl.rp.qos, ctx->bpe_on ? sl.rp.bpe : nullptr,

@@ -425,7 +425,8 @@ int arks_select_slot(arks_ctx* ctx, int slot);
 /* per-kernel device timing of the last run_* call: CUDA events around every launch on the library's stream.
  * arks_last_kernel_ms returns the number of intervals and fills ms[]: after a request batch {scan stage, rank_hot +
  * limit_admit, the fast-path kernel of the two-stage scan alone (0: fused kernel), the BPE kernels (0: no vocabulary)},
- * after a response batch {scan stage, fast-path kernel alone, BPE kernels}. */
+ * after a response batch {scan stage, fast-path kernel alone, BPE kernels}. The head kernel each run starts with (the window
+ * roll and the clears) lies outside every interval; the event records serialize the kernels they sit between. */
 int arks_set_profiling(arks_ctx* ctx, int on);
 int arks_last_kernel_ms(arks_ctx* ctx, float* ms, int cap);
 /* CUDA stream handle (cudaStream_t) the kernels are launched on, for event timing by the caller */
