@@ -240,11 +240,15 @@ constexpr uint8_t PS_STREAM = 1;     // "stream": true
 constexpr uint8_t PS_STREAM_OK = 2;  // stream_options.include_usage == true
 constexpr uint8_t PS_BAD = 0x40;     // the body does not decode (400 x-error-request-body-processing)
 
+// The fast path's body loads carry an L2 prefetch-size hint of 256 bytes: a lane reads its document 32 bytes per step, so
+// the first step into each aligned 256-byte block brings the block's other seven chunks from HBM into L2 with it, and
+// those loads wait for L2 instead of HBM. Bodies are packed back to back, so the bytes it brings past a body's end are the
+// next body's.
 // one 32-byte chunk (one sector): sm_90 has no 256-bit load, so two 128-bit loads issued back to back, with no bound check
 // between them. p must be 32-byte aligned
 __device__ __forceinline__ void ld_nc_v8(const uint4* p, uint4& a, uint4& b) {
-  asm volatile("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%8];\n\t"
-               "ld.global.nc.v4.u32 {%4,%5,%6,%7}, [%8+16];"
+  asm volatile("ld.global.nc.L2::256B.v4.u32 {%0,%1,%2,%3}, [%8];\n\t"
+               "ld.global.nc.L2::256B.v4.u32 {%4,%5,%6,%7}, [%8+16];"
                : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w), "=r"(b.x), "=r"(b.y), "=r"(b.z), "=r"(b.w)
                : "l"(p));
 }

@@ -14,8 +14,9 @@
 //            chunk and walks its tokens through the JSON grammar, (d) the lanes that meet a member the gateway reads
 //            (model / stream / stream_options / usage) extract it.
 //
-// As a THROUGHPUT path it loses (its warp collectives and single-lane sections cost more instructions than a
-// lane-per-document scan) — large batches take mask_scan.cuh. Same contract as mask_scan.cuh: a
+// As a THROUGHPUT path it loses: per document, its warp collectives cost more than a lane-per-document scan, and that holds
+// with the single-lane tails taken out too (DESIGN.md §5, "Why large batches do not take it"). Large batches take
+// mask_scan.cuh. Same contract as mask_scan.cuh: a
 // FILTER in front of the exact engine (json_engine.cuh) that accepts a document only inside a conservative subset (valid
 // RFC 8259, no control bytes in strings, depth <= 32, top-level object, the members the gateway reads of the expected type,
 // not duplicated, spelled without escapes, <= kFastMaxLen bytes / kFastMaxTok structure bytes); everything else goes to
