@@ -10,10 +10,12 @@ from dataclasses import dataclass
 
 import numpy as np
 
-# enum arks_rule / arks_quota_type  (rate_limiter.go:31-68, arksquota_types.go:28-33 of the reference)
+# enum arks_rule / arks_quota_type  (rate_limiter.go:31-68, arksquota_types.go:28-33 of the reference; "cost" is this
+# project's: spend at the endpoints' prices, include/arks_gateway.h ARKS_QT_COST)
 RULES = {"rpm": 0, "rpd": 1, "tpm": 2, "tpd": 3}
 RULE_NAMES = ["rpm", "rpd", "tpm", "tpd"]
-QUOTA_TYPES = {"prompt": 0, "response": 1, "total": 2}
+QUOTA_TYPES = {"prompt": 0, "response": 1, "total": 2, "cost": 3}
+QT_COST = QUOTA_TYPES["cost"]
 QUOTA_NONE, QUOTA_MISSING = -1, -2
 GEN_HISTORY = 16  # ARKS_GEN_HISTORY: generations a response row can be re-mapped from
 

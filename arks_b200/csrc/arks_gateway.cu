@@ -10,6 +10,7 @@
 //                               zeroes rate[rule][*] when floor(now/W) advances, which is what a new Redis key is
 //     rate[4+rule][qos] int64   the window before it (0 when time skipped it), read by the sliding window only
 //     quota[quota][3]   int64   cumulative usage, never reset (quota/redis_impl.go:38-48)
+//     quota_cost[quota] int64   cumulative usage of the `cost` items (ARKS_QT_COST), billed at qos_price
 //   per batch: bodies (16-byte aligned spans), tokens, a batch-local group table (qos -> arrivals), results.
 //
 // Kernels (DESIGN.md section 5; which scan kernel takes a batch depends on its size only)
@@ -81,6 +82,7 @@ struct DevTables {
   const int32_t* qos_quota;
   const int32_t* qos_ep;  // endpoint index for (token namespace, model) or -1
   const uint8_t* qos_vocab;  // BPE vocabulary slot of the entry's model (arks_bind_model_vocab; 0: the default)
+  const long long* qos_price; // [n_qos][2] prompt / completion price of the entry's endpoint; null: the generation has no cost item
   const uint32_t* qos_rl_off;
   const uint8_t* rl_rule;
   const int64_t* rl_value;
@@ -94,6 +96,7 @@ struct DevTables {
   // state
   long long* rate;   // [8][n_qos]: planes 0..3 the current window of each rule, 4..7 the previous one
   long long* quota;  // [n_quotas][3]
+  long long* quota_cost;  // [n_quotas] the cost column (read and billed only when qos_price is set)
   long long* qdelta; // [n_quotas][3] increments not yet folded into the other GPUs' copies, or null (single-owner keys)
   long long* metrics; // [n_qos][ARKS_METRIC_COLS] Prometheus series (include/arks_gateway.h), or null when not enabled
   uint32_t n_qos;
@@ -1315,6 +1318,7 @@ __global__ void __launch_bounds__(128) limit_admit_kernel(DevTables T, ReqDev B)
     i0 = T.quota_item_off[qs]; i1 = T.quota_item_off[qs + 1];
     b0 = T.ep_backend_off[es]; b1 = T.ep_backend_off[es + 1];
     const long long qu0 = T.quota[(size_t)qs * 3], qu1 = T.quota[(size_t)qs * 3 + 1], qu2 = T.quota[(size_t)qs * 3 + 2];
+    const long long qu3 = T.qos_price ? T.quota_cost[qs] : 0;  // ARKS_QT_COST (no cost item in the generation: never read)
     if (B.sliding) {  // prev lives in planes 4..7 and changes only between batches (roll_windows, the generation carry)
       long long pv[4];
 #pragma unroll
@@ -1341,7 +1345,7 @@ __global__ void __launch_bounds__(128) limit_admit_kernel(DevTables T, ReqDev B)
     if (qt >= 0) {
       for (uint32_t j = i0; j < i1; j++) {
         const int ty = T.qitem_type[j];
-        const long long c = ty == 0 ? qu0 : ty == 1 ? qu1 : qu2;
+        const long long c = ty == 0 ? qu0 : ty == 1 ? qu1 : ty == 2 ? qu2 : qu3;
         if (c > T.qitem_value[j]) { quota_fail = (int)(j - i0); q_cur = c; q_lim = T.qitem_value[j]; break; }
       }
     }
@@ -1506,6 +1510,13 @@ __device__ __forceinline__ QosAcct load_qos_acct(const DevTables& T, int32_t qos
     }
   return a;
 }
+// ARKS_QT_COST items of quota qt (each bills the cost once). Read when billing in a generation with a cost item, not kept in
+// QosAcct, so that the accounting shape the scan kernels hold across their passes does not grow
+__device__ __forceinline__ unsigned long long cost_items(const DevTables& T, int32_t qt) {
+  uint32_t nc = 0;
+  for (uint32_t j = T.quota_item_off[qt]; j < T.quota_item_off[qt + 1]; j++) nc += T.qitem_type[j] == ARKS_QT_COST;
+  return nc;
+}
 
 // A11 for one response per lane (all 32 lanes must call): doTokenRateLimit / doTokenQuotaLimit and the result row.
 // bucket of gateway_token_distribution (ExponentialBuckets(1, 2, 17) + Inf): the first upper bound >= v
@@ -1557,6 +1568,13 @@ __device__ __forceinline__ void account_usage(const DevTables& T, const RespDev&
 #pragma unroll
     for (int ty = 0; ty < 3; ty++)
       warp_agg_add(T.qdelta + (size_t)(qt >= 0 ? qt : 0) * 3 + ty, add[ty], counted && qt >= 0 && add[ty] != 0);
+  }
+  if (T.qos_price) {  // ARKS_QT_COST: prompt x p_prompt + completion x p_completion per cost item, modulo 2^64
+    const unsigned long long nc = counted && qt >= 0 ? cost_items(T, qt) : 0ull;
+    const unsigned long long cost = nc ? ((unsigned long long)u0 * (unsigned long long)T.qos_price[2 * (size_t)qos] +
+                                          (unsigned long long)u1 * (unsigned long long)T.qos_price[2 * (size_t)qos + 1]) * nc
+                                       : 0ull;
+    warp_agg_add(T.quota_cost + (qt >= 0 ? qt : 0), (long long)cost, cost != 0);
   }
   if (live) {
     B.reason[i] = reason;
@@ -2020,35 +2038,45 @@ __global__ void __launch_bounds__(128) meter_charge_kernel(DevTables T, uint32_t
     warp_agg_add(T.qdelta + qrow + side, add_side, q_on && add_side != 0);
     warp_agg_add(T.qdelta + qrow + 2, add_total, q_on && add_total != 0);
   }
+  if (T.qos_price) {  // ARKS_QT_COST: the count at the side's price, once per cost item
+    const unsigned long long nc = q_on ? cost_items(T, a.qt) : 0ull;
+    const long long add_cost = nc ? (long long)((unsigned long long)c * (unsigned long long)T.qos_price[2 * (size_t)qos + side] * nc) : 0;
+    warp_agg_add(T.quota_cost + (q_on ? a.qt : 0), add_cost, add_cost != 0);
+  }
   if (T.metrics) warp_agg_add(T.metrics + (size_t)row * ARKS_METRIC_COLS + ARKS_METRIC_USAGE + side, c, on);
 }
 
-// syncQuotaUsage (arks_impl.go:226-296): one lane per ArksQuota, in place on the device copies of the CR status
-__global__ void sync_quota_kernel(const uint32_t* item_off, const uint8_t* item_type, long long* quota, uint32_t n_quotas, int restore,
-                                  uint32_t* present, long long* used, uint8_t* action) {
+// syncQuotaUsage (arks_impl.go:226-296): one lane per ArksQuota, in place on the device copies of the CR status. cost null: the
+// three token columns, status_used [n][3], cost items ignored; else also the cost column (type 3), status_used [n][4]
+__global__ void sync_quota_kernel(const uint32_t* item_off, const uint8_t* item_type, long long* quota, long long* cost, uint32_t n_quotas,
+                                  int restore, uint32_t* present, long long* used, uint8_t* action) {
   const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= n_quotas) return;
+  const uint32_t cols = cost ? 4u : 3u;
   uint32_t pres = present[q];
-  long long u[3] = {used[3 * (size_t)q], used[3 * (size_t)q + 1], used[3 * (size_t)q + 2]};
-  long long* cur = quota + 3 * (size_t)q;
+  long long u[4] = {used[cols * (size_t)q], used[cols * (size_t)q + 1], used[cols * (size_t)q + 2], cost ? used[4 * (size_t)q + 3] : 0};
+  long long* row[4] = {quota + 3 * (size_t)q, quota + 3 * (size_t)q + 1, quota + 3 * (size_t)q + 2, cost ? cost + q : nullptr};
   int update_cr = 0, update_quota = 0;
   for (uint32_t j = item_off[q]; j < item_off[q + 1]; j++) {
     const int ty = item_type[j];
+    if (ty >= (int)cols) continue;
+    const long long cur = *row[ty];
     if (pres & (1u << ty)) {
-      if (u[ty] < cur[ty]) { update_cr = 1; u[ty] = cur[ty]; }
-      else if (u[ty] > cur[ty]) update_quota = 1;
+      if (u[ty] < cur) { update_cr = 1; u[ty] = cur; }
+      else if (u[ty] > cur) update_quota = 1;
     } else {
-      update_cr = 1; pres |= 1u << ty; u[ty] = cur[ty];
+      update_cr = 1; pres |= 1u << ty; u[ty] = cur;
     }
   }
   if (update_quota)
     for (uint32_t j = item_off[q]; j < item_off[q + 1]; j++) {
       const int ty = item_type[j];
-      if (!restore) cur[ty] = 0;  // SetUsage(QosToQuotaRequests(conf, nil)): Request == 0
-      else if (u[ty] > cur[ty]) cur[ty] = u[ty];
+      if (ty >= (int)cols) continue;
+      if (!restore) *row[ty] = 0;  // SetUsage(QosToQuotaRequests(conf, nil)): Request == 0
+      else if (u[ty] > *row[ty]) *row[ty] = u[ty];
     }
   present[q] = pres;
-  used[3 * (size_t)q] = u[0]; used[3 * (size_t)q + 1] = u[1]; used[3 * (size_t)q + 2] = u[2];
+  for (uint32_t c = 0; c < cols; c++) used[cols * (size_t)q + c] = u[c];
   action[q] = (uint8_t)(update_cr | update_quota << 1);
 }
 
@@ -2127,6 +2155,9 @@ struct arks_ctx {
   long long* d_metrics = nullptr;  // [n_qos][ARKS_METRIC_COLS] when metrics are enabled
   bool metrics_on = false;
   long long* d_quota = nullptr;
+  long long* d_quota_cost = nullptr;  // [n_quotas] the cost column (ARKS_QT_COST), carried by key like d_quota
+  bool has_cost = false;              // the current generation has a cost item (under cfg_mu)
+  std::unordered_map<std::string, std::pair<int64_t, int64_t>> ep_price;  // namespace \0 endpoint -> prices (arks_set_endpoint_price), under cfg_mu
   long long* d_qdelta = nullptr;   // allocated when quota sharing is enabled
   long long* d_qtmp = nullptr;
   long long* d_qexp = nullptr;     // what the last arks_export_quota_delta_dev handed out
@@ -2445,29 +2476,37 @@ int64_t arks_last_declined(arks_ctx* ctx) {
 uint64_t arks_launch_count(const arks_ctx* ctx) { return ctx ? ctx->launches : 0; }
 int arks_last_staging_route(const arks_ctx* ctx) { return ctx ? ctx->last_route : -1; }
 
-int arks_sync_quota_usage(arks_ctx* ctx, int mode, uint32_t* status_present, int64_t* status_used, uint8_t* action) {
+static int sync_quota(arks_ctx* ctx, int mode, uint32_t* status_present, int64_t* status_used, uint8_t* action, bool with_cost) {
   if (!ctx || !ctx->loaded) return ARKS_E_NOT_LOADED;
   if (!status_present || !status_used || !action || (mode != ARKS_SYNC_REFERENCE && mode != ARKS_SYNC_RESTORE)) return ARKS_E_INVALID_ARG;
   const uint32_t n = ctx->ht.n_quotas;
   if (n == 0) return 0;
+  const size_t cols = with_cost ? 4 : 3;
   CK(cudaSetDevice(ctx->device));
   uint32_t* d_pres = nullptr;
   long long* d_used = nullptr;
   uint8_t* d_act = nullptr;
   CK(cudaMalloc(&d_pres, (size_t)4 * n));
-  CK(cudaMalloc(&d_used, (size_t)24 * n));
+  CK(cudaMalloc(&d_used, 8 * cols * n));
   CK(cudaMalloc(&d_act, n));
   CK(cudaMemcpyAsync(d_pres, status_present, (size_t)4 * n, cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemcpyAsync(d_used, status_used, (size_t)24 * n, cudaMemcpyHostToDevice, ctx->stream));
-  sync_quota_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(ctx->dt.quota_item_off, ctx->dt.qitem_type, ctx->d_quota, n,
-                                                            mode == ARKS_SYNC_RESTORE, d_pres, d_used, d_act);
+  CK(cudaMemcpyAsync(d_used, status_used, 8 * cols * n, cudaMemcpyHostToDevice, ctx->stream));
+  sync_quota_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(ctx->dt.quota_item_off, ctx->dt.qitem_type, ctx->d_quota,
+                                                            with_cost ? ctx->d_quota_cost : nullptr, n, mode == ARKS_SYNC_RESTORE,
+                                                            d_pres, d_used, d_act);
   CK(cudaMemcpyAsync(status_present, d_pres, (size_t)4 * n, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaMemcpyAsync(status_used, d_used, (size_t)24 * n, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(status_used, d_used, 8 * cols * n, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaMemcpyAsync(action, d_act, n, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   cudaFree(d_pres); cudaFree(d_used); cudaFree(d_act);
   ctx->launches += 1;
   return 0;
+}
+int arks_sync_quota_usage(arks_ctx* ctx, int mode, uint32_t* status_present, int64_t* status_used, uint8_t* action) {
+  return sync_quota(ctx, mode, status_present, status_used, action, false);
+}
+int arks_sync_quota_usage_with_cost(arks_ctx* ctx, int mode, uint32_t* status_present, int64_t* status_used, uint8_t* action) {
+  return sync_quota(ctx, mode, status_present, status_used, action, true);
 }
 
 int arks_enable_metrics(arks_ctx* ctx, int on) {
@@ -2679,9 +2718,15 @@ static int queue_meter(arks_ctx* ctx, uint32_t n, const uint8_t* reason, const u
 // ---- config plane -------------------------------------------------------------------------------
 // Counters of the outgoing generation carried into the incoming one ON THE DEVICE, stream-ordered between two batches:
 // row q of the new arrays is row map[q] of the old ones (or zero). No host round trip, no stream synchronisation.
+// dst1 / src1 (may be null): one more [n_new] column carried by the same map in the same launch (the quota cost column)
 __global__ void carry_rows_kernel(long long* dst, const long long* src, const int32_t* map, uint32_t n_new, uint32_t cols, uint32_t dst_stride,
-                                  uint32_t src_stride, int col_major) {
+                                  uint32_t src_stride, int col_major, long long* dst1, const long long* src1) {
   const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (dst1 && k >= n_new * cols && k < n_new * (cols + 1)) {
+    const int32_t o = map[k - n_new * cols];
+    dst1[k - n_new * cols] = o < 0 ? 0 : src1[o];
+    return;
+  }
   if (k >= n_new * cols) return;
   const uint32_t q = col_major ? k % n_new : k / cols, c = col_major ? k / n_new : k % cols;
   const int32_t o = map[q];
@@ -2696,8 +2741,9 @@ struct arks_prepared {
   HostTables ht;
   std::vector<void*> allocs;  // tables; freed when the generation is retired
   DevTables d{};
-  long long *rate = nullptr, *quota = nullptr, *metrics = nullptr, *qdelta = nullptr, *qtmp = nullptr, *qexp = nullptr;
+  long long *rate = nullptr, *quota = nullptr, *quota_cost = nullptr, *metrics = nullptr, *qdelta = nullptr, *qtmp = nullptr, *qexp = nullptr;
   int32_t *d_qos_from = nullptr, *d_quota_from = nullptr;  // new row -> old row, on the device
+  bool has_cost = false;  // a quota of this generation has a cost item
   std::vector<int32_t> old_to_new;                          // qos index of the outgoing generation -> this one
   uint32_t base_generation = 0;
   uint32_t n_qos = 0, n_quotas = 0;
@@ -2723,10 +2769,10 @@ int arks_prepare_tables(arks_ctx* ctx, const arks_tables* t, arks_prepared** out
   auto S = [&](uint32_t id) {
     return std::string((const char*)t->str_bytes + t->str_off[id], t->str_off[id + 1] - t->str_off[id]);
   };
-  for (uint32_t i = 0; i < t->n_rl; i++)
-    if (t->rl_rule[i] >= ARKS_N_RULES) return fail(ctx, ARKS_E_BAD_TABLE, "unknown rate-limit rule %u", t->rl_rule[i]);
-  for (uint32_t i = 0; i < t->n_qitems; i++)
-    if (t->qitem_type[i] >= ARKS_N_QT) return fail(ctx, ARKS_E_BAD_TABLE, "unknown quota type %u", t->qitem_type[i]);
+  bool has_cost = false;
+  for (uint32_t i = 0; i < t->n_qitems; i++) has_cost |= t->qitem_type[i] == ARKS_QT_COST;
+  if (has_cost && ctx->share_quota)
+    return fail(ctx, ARKS_E_INVALID_ARG, "cost quota items cannot be used with quota sharing across GPUs (the fold carries token items only)");
   for (uint32_t q = 0; q < t->n_qos; q++) {
     if (t->qos_rl_off[q + 1] - t->qos_rl_off[q] > 255) return fail(ctx, ARKS_E_BAD_TABLE, "more than 255 rate limits");
     if (t->qos_quota[q] >= (int32_t)t->n_quotas || t->qos_quota[q] < ARKS_QUOTA_MISSING)
@@ -2793,6 +2839,7 @@ int arks_prepare_tables(arks_ctx* ctx, const arks_tables* t, arks_prepared** out
   std::vector<int32_t> old_to_new;  // qos index of the outgoing generation -> this one
   uint32_t base_generation;
   std::unordered_map<std::string, uint32_t> vocab_bind;  // model name -> BPE vocabulary slot, as bound now
+  std::vector<long long> qos_price;                      // [n_qos][2] when the generation has a cost item
   {
     // the only part that looks at the current generation: short, so that a commit on the batch thread never waits for
     // the tens of milliseconds a prepare on the config thread takes
@@ -2800,6 +2847,17 @@ int arks_prepare_tables(arks_ctx* ctx, const arks_tables* t, arks_prepared** out
     base_generation = ctx->generation;
     vocab_bind = ctx->vocab_bind;
     old_to_new.assign(ctx->loaded ? ctx->ht.n_qos : 0, -1);
+    // the price of every qos entry: that of the endpoint its (token namespace, model) resolves to, as priced now
+    if (has_cost) {
+      qos_price.assign((size_t)2 * t->n_qos, 0);
+      for (uint32_t q = 0; q < t->n_qos; q++) {
+        if (qos_ep[q] < 0 || ctx->ep_price.empty()) continue;
+        auto it = ctx->ep_price.find(S(t->ep_ns_str[qos_ep[q]]) + '\0' + S(t->ep_name_str[qos_ep[q]]));
+        if (it == ctx->ep_price.end()) continue;
+        qos_price[2 * (size_t)q] = it->second.first;
+        qos_price[2 * (size_t)q + 1] = it->second.second;
+      }
+    }
   if (ctx->loaded) {
     std::unordered_map<std::string, uint32_t> oq, ou;
     for (uint32_t q = 0; q < ctx->ht.n_qos; q++) oq.emplace(ctx->ht.qos_key[q], q);
@@ -2870,6 +2928,7 @@ int arks_prepare_tables(arks_ctx* ctx, const arks_tables* t, arks_prepared** out
   PUT(v_qos_quota, qos_quota);
   PUT(qos_ep, qos_ep);
   PUT(qos_vocab, qos_vocab);
+  if (has_cost) PUT(qos_price, qos_price);
   PUT(v_qos_rl_off, qos_rl_off);
   PUT(v_rl_rule, rl_rule);
   PUT(v_rl_value, rl_value);
@@ -2878,12 +2937,13 @@ int arks_prepare_tables(arks_ctx* ctx, const arks_tables* t, arks_prepared** out
   PUT(v_qi_val, qitem_value);
   PUT(v_ep_off, ep_backend_off);
   PUT(v_bw, backend_weight);
-  long long *n_rate = nullptr, *n_quota = nullptr, *n_metrics = nullptr, *n_qdelta = nullptr, *n_qtmp = nullptr, *n_qexp = nullptr;
+  long long *n_rate = nullptr, *n_quota = nullptr, *n_quota_cost = nullptr, *n_metrics = nullptr, *n_qdelta = nullptr, *n_qtmp = nullptr, *n_qexp = nullptr;
   int32_t *n_qos_from = nullptr, *n_quota_from = nullptr;
   {
     int rc;
     if ((rc = put(nullptr, 0, (void**)&n_rate, (size_t)64 * t->n_qos))) return rc;  // [8][n_qos]: current and previous windows
     if ((rc = put(nullptr, 0, (void**)&n_quota, (size_t)24 * t->n_quotas))) return rc;
+    if ((rc = put(nullptr, 0, (void**)&n_quota_cost, (size_t)8 * t->n_quotas))) return rc;
     if ((rc = put(nullptr, 0, (void**)&n_metrics, (size_t)8 * ARKS_METRIC_COLS * t->n_qos))) return rc;
     if ((rc = put(qos_from.data(), (size_t)4 * (t->n_qos + 1), (void**)&n_qos_from))) return rc;
     if ((rc = put(quota_from.data(), (size_t)4 * (t->n_quotas + 1), (void**)&n_quota_from))) return rc;
@@ -2921,7 +2981,7 @@ int arks_prepare_tables(arks_ctx* ctx, const arks_tables* t, arks_prepared** out
   }
   arks_prepared* p = new arks_prepared();
   p->allocs = fresh;
-  p->rate = n_rate; p->quota = n_quota; p->metrics = n_metrics; p->qdelta = n_qdelta; p->qtmp = n_qtmp; p->qexp = n_qexp;
+  p->rate = n_rate; p->quota = n_quota; p->quota_cost = n_quota_cost; p->has_cost = has_cost; p->metrics = n_metrics; p->qdelta = n_qdelta; p->qtmp = n_qtmp; p->qexp = n_qexp;
   p->d_qos_from = n_qos_from; p->d_quota_from = n_quota_from;
   d.n_qos = t->n_qos;
   p->d = d;
@@ -2947,22 +3007,24 @@ int arks_commit_tables(arks_ctx* ctx, arks_prepared* p) {
   if (p->vocab_used & ~ctx->vocab_loaded)
     return fail(ctx, ARKS_E_INVALID_ARG, "prepared with a BPE vocabulary slot that has been emptied since: prepare again");
   if (ctx->loaded) {
-    auto carry = [&](long long* dst, const long long* src, const int32_t* map, uint32_t n_new, uint32_t cols, uint32_t ds, uint32_t ss, int cm) {
+    auto carry = [&](long long* dst, const long long* src, const int32_t* map, uint32_t n_new, uint32_t cols, uint32_t ds, uint32_t ss, int cm,
+                     long long* dst1 = nullptr, const long long* src1 = nullptr) {
       if (!dst || !src || !n_new) return;
-      const uint32_t total = n_new * cols;
-      carry_rows_kernel<<<(total + 255) / 256, 256, 0, ctx->stream>>>(dst, src, map, n_new, cols, ds, ss, cm);
+      const uint32_t total = n_new * (cols + (dst1 ? 1 : 0));
+      carry_rows_kernel<<<(total + 255) / 256, 256, 0, ctx->stream>>>(dst, src, map, n_new, cols, ds, ss, cm, dst1, src1);
       ctx->launches += 1;
     };
     carry(p->rate, ctx->d_rate, p->d_qos_from, p->n_qos, 8, p->n_qos, ctx->ht.n_qos, 1);  // both windows, by key
     carry(p->metrics, ctx->d_metrics, p->d_qos_from, p->n_qos, ARKS_METRIC_COLS, 0, 0, 0);
-    carry(p->quota, ctx->d_quota, p->d_quota_from, p->n_quotas, 3, 0, 0, 0);
+    carry(p->quota, ctx->d_quota, p->d_quota_from, p->n_quotas, 3, 0, 0, 0, p->quota_cost, ctx->d_quota_cost);  // with the cost column
     carry(p->qdelta, ctx->d_qdelta, p->d_quota_from, p->n_quotas, 3, 0, 0, 0);
     CK(cudaGetLastError());
   }
   // retire the outgoing generation: freed stream-ordered, after the carry kernels and everything queued before them
   for (void* q : ctx->table_allocs) cudaFreeAsync(q, ctx->stream);  // the one arena of the outgoing generation
   ctx->table_allocs = std::move(p->allocs);
-  ctx->d_rate = p->rate; ctx->d_quota = p->quota; ctx->d_metrics = p->metrics;
+  ctx->d_rate = p->rate; ctx->d_quota = p->quota; ctx->d_quota_cost = p->quota_cost; ctx->d_metrics = p->metrics;
+  ctx->has_cost = p->has_cost;
   ctx->d_qdelta = p->qdelta; ctx->d_qtmp = p->qtmp; ctx->d_qexp = p->qexp;
   ctx->d_qos_from = p->d_qos_from; ctx->d_quota_from = p->d_quota_from;
   ctx->qexp_valid = false;
@@ -2971,6 +3033,7 @@ int arks_commit_tables(arks_ctx* ctx, arks_prepared* p) {
   d.rate = ctx->d_rate;
   d.metrics = ctx->metrics_on ? ctx->d_metrics : nullptr;
   d.quota = ctx->d_quota;
+  d.quota_cost = ctx->d_quota_cost;
   d.qdelta = ctx->d_qdelta;
   ctx->dt = d;
   if (ctx->loaded) {
@@ -3081,6 +3144,16 @@ int32_t arks_find_qos(const arks_ctx* ctx, const char* ns, uint32_t ns_len, cons
 }
 
 uint32_t arks_table_generation(const arks_ctx* ctx) { return ctx ? ctx->generation : 0; }
+int arks_set_endpoint_price(arks_ctx* ctx, const char* ns, uint32_t ns_len, const char* name, uint32_t name_len, int64_t prompt,
+                            int64_t completion) {
+  if (!ctx || !str_ok(ns, ns_len) || !str_ok(name, name_len)) return ARKS_E_INVALID_ARG;
+  if (prompt < 0 || completion < 0) return fail(ctx, ARKS_E_INVALID_ARG, "arks_set_endpoint_price: negative price");
+  std::lock_guard<std::mutex> g(ctx->cfg_mu);
+  const std::string k = std::string(ns ? ns : "", ns_len) + '\0' + std::string(name ? name : "", name_len);
+  if (prompt == 0 && completion == 0) ctx->ep_price.erase(k);
+  else ctx->ep_price[k] = {prompt, completion};
+  return 0;
+}
 int arks_set_precharge(arks_ctx* ctx, int on) {
   if (!ctx) return ARKS_E_INVALID_ARG;
   ctx->precharge = on != 0;
@@ -3873,6 +3946,14 @@ int arks_snapshot_quota(arks_ctx* ctx, int64_t* usage) {
   if (ctx->ht.n_quotas) CK(cudaMemcpy(usage, ctx->d_quota, (size_t)24 * ctx->ht.n_quotas, cudaMemcpyDeviceToHost));
   return 0;
 }
+int arks_snapshot_quota_cost(arks_ctx* ctx, int64_t* cost) {
+  if (!ctx || !ctx->loaded) return ARKS_E_NOT_LOADED;
+  if (!cost) return ARKS_E_INVALID_ARG;
+  CK(cudaSetDevice(ctx->device));
+  CK(cudaStreamSynchronize(ctx->stream));
+  if (ctx->ht.n_quotas) CK(cudaMemcpy(cost, ctx->d_quota_cost, (size_t)8 * ctx->ht.n_quotas, cudaMemcpyDeviceToHost));
+  return 0;
+}
 int arks_set_quota_usage(arks_ctx* ctx, uint32_t quota, const int64_t usage[3]) {
   if (!ctx || !ctx->loaded) return ARKS_E_NOT_LOADED;
   if (quota >= ctx->ht.n_quotas) return ARKS_E_INVALID_ARG;
@@ -3929,6 +4010,11 @@ int arks_snapshot_rate_prev(arks_ctx* ctx, int64_t now_unix, int64_t* counters) 
 // staleness, the same class of over-admission the reference's non-atomic Redis path has).
 int arks_enable_quota_sharing(arks_ctx* ctx, int on) {
   if (!ctx) return ARKS_E_INVALID_ARG;
+  {
+    std::lock_guard<std::mutex> g(ctx->cfg_mu);
+    if (on && ctx->has_cost)
+      return fail(ctx, ARKS_E_INVALID_ARG, "the current generation has cost quota items, which cannot be shared across GPUs");
+  }
   if (ctx->loaded) return fail(ctx, ARKS_E_INVALID_ARG, "enable quota sharing before arks_load_tables");
   ctx->share_quota = on != 0;
   return 0;

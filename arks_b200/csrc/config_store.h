@@ -101,6 +101,10 @@ inline const char* tables_shape_error(const arks_tables* t) {
   if (!ids(t->quota_ns_str, t->n_quotas) || !ids(t->quota_name_str, t->n_quotas)) return "ArksQuota: string id out of range";
   if (!csr(t->quota_item_off, t->n_quotas, t->n_qitems)) return "quota_item_off is not a CSR over the quota items";
   if (t->n_qitems && (!t->qitem_type || !t->qitem_value)) return "quota items: null pointer";
+  for (uint32_t i = 0; i < t->n_rl; i++)
+    if (t->rl_rule[i] >= ARKS_N_RULES) return "unknown rate-limit rule";
+  for (uint32_t i = 0; i < t->n_qitems; i++)
+    if (t->qitem_type[i] > ARKS_QT_COST) return "unknown quota type";
   if (!ids(t->ep_ns_str, t->n_endpoints) || !ids(t->ep_name_str, t->n_endpoints)) return "ArksEndpoint: string id out of range";
   if (!csr(t->ep_backend_off, t->n_endpoints, t->n_backends)) return "ep_backend_off is not a CSR over the backends";
   if (t->n_backends && !t->backend_weight) return "backend_weight: null pointer";

@@ -101,6 +101,9 @@ def lib():
         L.arks_snapshot_rate.argtypes = [vp, C.c_int64, abi.i64p]
         L.arks_snapshot_rate_prev.argtypes = [vp, C.c_int64, abi.i64p]
         L.arks_sync_quota_usage.argtypes = [vp, C.c_int, abi.u32p, abi.i64p, abi.u8p]
+        L.arks_sync_quota_usage_with_cost.argtypes = [vp, C.c_int, abi.u32p, abi.i64p, abi.u8p]
+        L.arks_snapshot_quota_cost.argtypes = [vp, abi.i64p]
+        L.arks_set_endpoint_price.argtypes = [vp, cp, u32, cp, u32, C.c_int64, C.c_int64]
         L.arks_enable_metrics.argtypes = [vp, C.c_int]
         L.arks_snapshot_metrics.argtypes = [vp, abi.i64p]
         L.arks_enable_quota_sharing.argtypes = [vp, C.c_int]
@@ -132,7 +135,7 @@ EXPORTED = [  # every symbol include/arks_gateway.h declares (checked by tests/t
     "arks_set_quota_usage", "arks_incr_quota_usage", "arks_snapshot_rate", "arks_snapshot_rate_prev", "arks_take_quota_delta",
     "arks_apply_quota_delta", "arks_quota_delta_dev", "arks_fold_quota_delta_dev", "arks_enable_quota_sharing",
     "arks_comm_unique_id", "arks_comm_init", "arks_comm_set_shared", "arks_fold_quota_allreduce", "arks_comm_destroy",
-    "arks_export_quota_delta_dev",
+    "arks_export_quota_delta_dev", "arks_set_endpoint_price", "arks_snapshot_quota_cost", "arks_sync_quota_usage_with_cost",
 ]
 
 
@@ -152,6 +155,7 @@ class Gateway:
                 lib().arks_destroy(h)
             raise ArksError(rc, msg)
         self.tables = None
+        self._priced = set()  # endpoints load_tables / prepare_tables gave a price (so a later snapshot can take it back)
         self.ratelimit_report = False
         self.sliding_window = False
 
@@ -171,13 +175,25 @@ class Gateway:
             raise ArksError(rc, lib().arks_last_error(self._h).decode())
 
     # ---- qosconfig.ConfigProvider: informer snapshot -> HBM tables
+    def _push_prices(self, tables):
+        """the spec.pricing of the snapshot's ArksEndpoints; an endpoint priced by an earlier snapshot and unpriced or absent in
+        this one loses its price"""
+        priced = {k: v for k, v in getattr(tables, "endpoint_price", {}).items() if v != (0, 0)}
+        for k in self._priced - priced.keys():
+            self.set_endpoint_price(k[0], k[1], 0, 0)
+        for k, (p, c) in priced.items():
+            self.set_endpoint_price(k[0], k[1], p, c)
+        self._priced = set(priced)
+
     def load_tables(self, tables):
+        self._push_prices(tables)
         ts = tables.c_struct()
         self._ck(lib().arks_load_tables(self._h, C.byref(ts)))
         self.tables = tables
 
     def prepare_tables(self, tables):
         """config thread: build + upload the next generation off the data path -> opaque handle for commit_tables"""
+        self._push_prices(tables)
         ts = tables.c_struct()
         h = C.c_void_p()
         self._ck(lib().arks_prepare_tables(self._h, C.byref(ts), C.byref(h)))
@@ -223,6 +239,12 @@ class Gateway:
         f = {"token": lib().arks_delete_token, "quota": lib().arks_delete_quota, "endpoint": lib().arks_delete_endpoint}[kind]
         ns, nm = namespace.encode(), name.encode()
         self._ck(f(self._h, ns, len(ns), nm, len(nm)))
+
+    def set_endpoint_price(self, namespace: str, name: str, prompt: int, completion: int):
+        """prices per token of ArksEndpoint namespace/name for `cost` quota items (>= 0; (0, 0) removes the price); read by the
+        next prepare / load, like every config-plane change"""
+        ns, nm = namespace.encode(), name.encode()
+        self._ck(lib().arks_set_endpoint_price(self._h, ns, len(ns), nm, len(nm), int(prompt), int(completion)))
 
     def config_prepare(self):
         h = C.c_void_p()
@@ -395,15 +417,23 @@ class Gateway:
         self._ck(lib().arks_snapshot_quota(self._h, abi.ptr(out, abi.i64p)))
         return out
 
+    def snapshot_quota_cost(self) -> np.ndarray:
+        """the cost column of every quota (usage of its `cost` items)"""
+        out = np.zeros(self.tables.n_quotas, np.int64)
+        self._ck(lib().arks_snapshot_quota_cost(self._h, abi.ptr(out, abi.i64p)))
+        return out
+
     def sync_quota_usage(self, status_present: np.ndarray, status_used: np.ndarray, restore: bool = False) -> np.ndarray:
         """syncQuotaUsage over all ArksQuotas (arks_impl.go:217-300). status_present [n_quotas] uint32 bit masks and
         status_used [n_quotas, 3] int64 are updated in place (the CR status to write back); returns action[n_quotas]:
-        bit0 update the CR, bit1 the store was outdated (reference: zeroed; restore=True: raised to the CR value)."""
+        bit0 update the CR, bit1 the store was outdated (reference: zeroed; restore=True: raised to the CR value).
+        status_used [n_quotas, 4]: the same pass over the cost column too (column 3, bit 3; arks_sync_quota_usage_with_cost)."""
         n = self.tables.n_quotas
-        assert status_present.dtype == np.uint32 and status_used.dtype == np.int64 and status_used.shape == (n, 3)
+        assert status_present.dtype == np.uint32 and status_used.dtype == np.int64 and status_used.shape in ((n, 3), (n, 4))
+        f = lib().arks_sync_quota_usage_with_cost if status_used.shape[1] == 4 else lib().arks_sync_quota_usage
         action = np.zeros(n, np.uint8)
-        self._ck(lib().arks_sync_quota_usage(self._h, 1 if restore else 0, abi.ptr(status_present, abi.u32p),
-                                             abi.ptr(status_used, abi.i64p), abi.ptr(action, abi.u8p)))
+        self._ck(f(self._h, 1 if restore else 0, abi.ptr(status_present, abi.u32p), abi.ptr(status_used, abi.i64p),
+                   abi.ptr(action, abi.u8p)))
         return action
 
     def enable_metrics(self, on: bool = True):

@@ -30,7 +30,7 @@ import time
 import numpy as np
 
 from . import abi
-from .tables import Tables, endpoint_backends
+from .tables import Tables, endpoint_backends, endpoint_pricing
 
 KINDS = {"ArksToken": "token", "ArksQuota": "quota", "ArksEndpoint": "endpoint"}
 QUOTA_TYPE_NAMES = sorted(abi.QUOTA_TYPES, key=abi.QUOTA_TYPES.get)
@@ -58,7 +58,7 @@ def _spec_of(kind, obj, ready_backends):
         return (obj["spec"]["token"], token_qos(obj))
     if kind == "quota":
         return quota_items(obj)
-    return endpoint_backends(obj, ready_backends)
+    return endpoint_backends(obj, ready_backends) + (endpoint_pricing(obj),)
 
 
 class ArksProvider:
@@ -121,6 +121,8 @@ class ArksProvider:
                 self.g.upsert_quota(k[0], k[1], spec)
             else:
                 self.g.upsert_endpoint(k[0], k[1], spec[1])
+                if spec[2] != self._price_of(k):
+                    self.g.set_endpoint_price(k[0], k[1], *spec[2])
         except Exception as e:  # the library keeps the previous version of the object
             self._reject(kind, k, e)
             return False
@@ -129,6 +131,11 @@ class ArksProvider:
         self.dirty = True
         return True
 
+    def _price_of(self, k):
+        """the price last pushed for endpoint k ((0, 0): none; only priced endpoints ever reach set_endpoint_price)"""
+        spec = self._spec["endpoint"].get(k)
+        return spec[2] if spec else (0, 0)
+
     def _reject(self, kind, k, e):
         self.rejected.append((kind, k, repr(e)))
         del self.rejected[:-256]  # a diagnostic, not a log: an object that is re-sent broken for days must not grow the process
@@ -136,6 +143,8 @@ class ArksProvider:
     def _delete(self, kind, obj) -> bool:
         k = object_key(obj)
         self.objects[kind].pop(k, None)
+        if kind == "endpoint" and self._price_of(k) != (0, 0):
+            self.g.set_endpoint_price(k[0], k[1], 0, 0)
         if self._spec[kind].pop(k, None) is None:
             self.ignored += 1
             return False
@@ -176,7 +185,7 @@ class ArksProvider:
             t = self.g.tables
             n = t.n_quotas
             present = np.zeros(n, np.uint32)
-            used = np.zeros((n, 3), np.int64)
+            used = np.zeros((n, len(QUOTA_TYPE_NAMES)), np.int64)  # the token columns and the cost column
             objs = []
             for q in range(n):
                 k = (t.strings[t.quota_ns_str[q]].decode(), t.strings[t.quota_name_str[q]].decode())

@@ -91,9 +91,15 @@ class Tables:
 
         e_ns, e_name, e_off, b_w = [], [], [0], []
         self.endpoint_backends: list[list[str]] = []
+        # (namespace, name) -> (prompt, completion) price per token of the priced endpoints (spec.pricing, `cost` quota items);
+        # Gateway.load_tables / prepare_tables hand them to the library. The first object wins on duplicates, as in the lookup
+        self.endpoint_price: dict[tuple[str, str], tuple[int, int]] = {}
         for e in endpoints:
             md = e["metadata"]
             ns = md.get("namespace", "default")
+            price = endpoint_pricing(e)
+            if price != (0, 0):
+                self.endpoint_price.setdefault((ns, md["name"]), price)
             e_ns.append(s(ns))
             e_name.append(s(md["name"]))
             names, weights = endpoint_backends(e, ready_backends)
@@ -168,6 +174,24 @@ def endpoint_backends(e, ready_backends=None):
     return names, weights
 
 
+def endpoint_pricing(e):
+    """(prompt, completion) of an ArksEndpoint's optional spec.pricing: integer prices per token in the unit of the `cost` quota
+    items (nano-dollars per token = dollars per 1M tokens x 1000); (0, 0) when absent. ValueError when a price is negative,
+    not an integer or out of int64 range"""
+    pr = (e.get("spec") or {}).get("pricing")
+    if pr is None:
+        return 0, 0
+    if not isinstance(pr, dict):
+        raise ValueError(f"spec.pricing must be an object, not {pr!r}")
+    out = []
+    for k in ("prompt", "completion"):
+        v = pr.get(k, 0)
+        if isinstance(v, bool) or not isinstance(v, int) or not 0 <= v < 2**63:
+            raise ValueError(f"spec.pricing.{k} must be an integer in [0, 2^63), not {v!r}")
+        out.append(v)
+    return out[0], out[1]
+
+
 def simple_token(name, namespace, token, model, limits, quota=""):
     """Convenience: one ArksToken with a single qos entry (limits: list of (type, value))."""
     return {"metadata": {"name": name, "namespace": namespace},
@@ -181,7 +205,10 @@ def simple_quota(name, namespace, items):
             "spec": {"quotas": [{"type": t, "value": v} for t, v in items]}}
 
 
-def simple_endpoint(name, namespace, default_weight=1, routes=()):
-    return {"metadata": {"name": name, "namespace": namespace},
-            "spec": {"defaultWeight": default_weight,
-                     "routeConfigs": [{"name": n, "weight": w} for n, w in routes]}}
+def simple_endpoint(name, namespace, default_weight=1, routes=(), pricing=None):
+    e = {"metadata": {"name": name, "namespace": namespace},
+         "spec": {"defaultWeight": default_weight,
+                  "routeConfigs": [{"name": n, "weight": w} for n, w in routes]}}
+    if pricing is not None:
+        e["spec"]["pricing"] = {"prompt": pricing[0], "completion": pricing[1]}
+    return e

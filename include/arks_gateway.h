@@ -50,7 +50,7 @@ enum arks_status {
   ARKS_E_NO_DEVICE = -2,
   ARKS_E_CUDA = -3,
   ARKS_E_TIME_WENT_BACK = -4, /* now_unix fell into an earlier window than a previous batch */
-  ARKS_E_BAD_TABLE = -5,      /* unknown rate-limit rule / quota type (reference: 500 / panic,
+  ARKS_E_BAD_TABLE = -5,      /* unknown rate-limit rule / quota type > ARKS_QT_COST (reference: 500 / panic,
                                  pkg/gateway/check.go:112-121, ratelimiter/types.go:46); or a snapshot whose
                                  offsets / string ids / weights are out of range (checked before anything follows them) */
   ARKS_E_CAPACITY = -6,
@@ -70,7 +70,9 @@ enum arks_quota_type {
   ARKS_QT_PROMPT = 0,
   ARKS_QT_RESPONSE = 1,
   ARKS_QT_TOTAL = 2,
-  ARKS_N_QT = 3,
+  ARKS_N_QT = 3,   /* the token-count types: quota usage rows are [n_quotas][ARKS_N_QT] */
+  ARKS_QT_COST = 3, /* spend in cost units, billed at the endpoint's prices (arks_set_endpoint_price); its usage is the
+                     * separate cost column (arks_snapshot_quota_cost). Not in the reference, whose QuotaType stops at total */
 };
 #define ARKS_QUOTA_NONE (-1)    /* qos.quota.name == ""           handle_request.go:185 */
 #define ARKS_QUOTA_MISSING (-2) /* named ArksQuota does not exist check.go:76-84 -> 500 */
@@ -479,6 +481,34 @@ int arks_set_quota_usage(arks_ctx* ctx, uint32_t quota, const int64_t usage[3]);
 int arks_sync_quota_usage(arks_ctx* ctx, int mode, uint32_t* status_present /* n_quotas */, int64_t* status_used /* 3 * n_quotas */,
                           uint8_t* action /* n_quotas */);
 int arks_incr_quota_usage(arks_ctx* ctx, uint32_t quota, const int64_t delta[3]); /* IncrUsage */
+
+/* ---- pricing-based quotas: the `cost` quota item (ARKS_QT_COST) ---------------------------------------------------------
+ * Token quotas cannot cap what a tenant spends once one ArksQuota is shared by qos entries of models with different prices.
+ * A `cost` item's value is a limit in cost units (nano-dollars per token = dollars per 1M tokens x 1000 keeps every price an
+ * integer). Semantics:
+ *   - checked at request time like every item, in spec order after the rate limits: usage > limit denies (usage == limit
+ *     admits), the first failing item gives ARKS_R_QUOTA with detail = its index and cur_usage / limit_max = the cost figures;
+ *   - billed wherever the token items are: a counted response adds prompt_tokens x p_prompt + completion_tokens x
+ *     p_completion; a metered stream (arks_set_stream_metering) adds its prompt's count x p_prompt when its batch commits and
+ *     each chunk's count x p_completion. Modulo 2^64 like every counter; a quota with n cost items adds n times (the
+ *     reference's convention of one INCRBY per item). ARKS_R_QOS_GONE rows bill nothing; the pre-charge does not touch it;
+ *   - prices are per ArksEndpoint (namespace, name). A qos entry is priced by the endpoint its (token namespace, model)
+ *     resolves to; no endpoint or no price: 0. Prices are config-plane state read by arks_prepare_tables / arks_load_tables /
+ *     arks_config_prepare: they take effect with the NEXT generation, and a response row is billed at the prices of the
+ *     generation it is billed in (the current one), like arks_bind_model_vocab;
+ *   - the cost usage of a quota is carried by (namespace, quotaName) across swaps, like the other items;
+ *   - not with quota sharing across GPUs: arks_prepare_tables refuses a generation with a cost item while sharing is on, and
+ *     arks_enable_quota_sharing refuses while the current generation has one.
+ * A generation without a cost item decides, counts and launches exactly as without this feature. */
+/* config thread: the prices per token of ArksEndpoint (ns, name); both >= 0, (0, 0) removes the price */
+int arks_set_endpoint_price(arks_ctx* ctx, const char* ns, uint32_t ns_len, const char* name, uint32_t name_len, int64_t prompt,
+                            int64_t completion);
+int arks_snapshot_quota_cost(arks_ctx* ctx, int64_t* cost /* n_quotas */);
+/* arks_sync_quota_usage over four columns: status_present bit 3 and status_used[4q + 3] are the cost item's, in one pass
+ * (ARKS_SYNC_REFERENCE zeroes every item of an outdated quota, the cost column included). The three-column call above
+ * leaves the cost column alone. */
+int arks_sync_quota_usage_with_cost(arks_ctx* ctx, int mode, uint32_t* status_present /* n_quotas */,
+                                    int64_t* status_used /* 4 * n_quotas */, uint8_t* action /* n_quotas */);
 /* rate counters of the CURRENT windows (value 0 if the stored window is older than now_unix's) */
 int arks_snapshot_rate(arks_ctx* ctx, int64_t now_unix, int64_t* counters /* 4 * n_qos */);
 /* rate counters of the windows just before now_unix's (what arks_set_sliding_window calls prev; 0 when not adjacent) */
